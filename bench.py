@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - interpolated frames/s of the RIFE-4.6 2x path at 1080p (BASELINE.json metric) on N B200s.
+"""bench.py - interpolated frames/s of the RIFE-4.6 2x path at 1080p (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one synthetic 64-frame 1080p clip per GPU (63 frame pairs, 2x ->
@@ -13,15 +13,22 @@ only exchange step).
   e2e   : same metric through the plugin call a ComfyUI user makes - RIFE_VFI().vfi(ckpt, frames, multiplier=2) - with a
           PAGEABLE [64,1080,1920,3] fp32 input tensor and the node's own output tensor; H2D + D2H (and the host-side
           staging and pass-through copies) inside the timed region.  e2e_capi is the same through the bare C-ABI call
-          on pre-pinned buffers (the r01 figure).
-  roofline     : the dominant kernel (tcgen05 tap-conv, block-3 ResConv layer) timed alone, against the measured
-                 bf16 tensor peak in MEASURED_PEAKS.json
+          on pre-pinned buffers.
+  roofline     : the dominant kernel (wgmma tap-conv, block-3 ResConv layer) timed alone, against the measured
+                 bf16 tensor peak in MEASURED_PEAKS.json (else the H100 SXM data sheet's dense figure)
   roofline_hbm : the HBM-bound kernels the step actually runs (block-3 / block-2 `front`, `final`), timed with CUDA
                  events on their launching stream inside real passes (vfi_rife_profile), against measured HBM bandwidth
   psnr_db      : the GPU's interpolated frames against the CPU leg's output on the CPU leg's sample of the same clip
   cpu_baseline : the CPU oracle port (oracle/rife46.py == the reference's PyTorch-CPU path, SURVEY.md F2) on the
                  host cores, on a bounded sample of the same clip (rank 0, N = 1 only)
 --impl reference times that CPU port alone (all host threads), same metric / config.
+--dump-outputs DIR writes what the timed path delivered in its last step as float32 .npy files: the interpolated frames
+on rank 0, i.e. for N > 1 every rank's frames as gathered there, in rank order (RIFE GPU path only; refused with
+--impl reference and the other workloads):
+  frames_first_last.npy  the first and the last interpolated frame of the step, [2, 1080, 1920, 3]
+  frames_sample.npy      3M values of the whole [frames, 1080, 1920, 3] output at fixed, seeded positions
+  The clip, the weights and the sample positions are seeded, so two builds run with the same arguments can be compared
+  output for output.
 """
 import argparse
 import json
@@ -42,8 +49,8 @@ FLOPS_PER_FRAME = 175.245e9          # SURVEY.md section 8d (87.62 GMAC)
 CPU_SAMPLE_FRAMES = 3                # 2 pairs of the same clip for the CPU legs (bounded sample)
 CPU_ARCH = "4.6"
 # N > 1: the shard's 63 pairs leave for rank 0 in this many chunks, each behind the kernels that produce it.  8 chunks = one
-# internal pass of 8 pairs per chunk (r02: 16 chunks of 4 pairs made every pass half as wide - the latency-bound blocks 0 / 1
-# cost the same per pass - and the step 4.7 ms slower than N = 1, whatever the transport)
+# internal pass of 8 pairs per chunk (smaller chunks make every pass narrower, and the latency-bound blocks 0 / 1 cost the
+# same per pass whatever its width)
 GATHER_CHUNKS = int(os.environ.get("VFI_GATHER_CHUNKS", "8"))
 
 
@@ -53,11 +60,12 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d["bf16_tflops"], tflops_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate; never reached, only bounds
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_sustained=None, source="H100 SXM data sheet (not measured)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read only: nvidia-smi --query-gpu)."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -121,7 +129,7 @@ class ClockSampler:
 def _pick_threads(sd):
     """Host thread count for the CPU legs: the fastest of a few candidates on a small (270x480) pair.  "All the
     host threads it can use" is not os.cpu_count() on these boxes: oneDNN conv with 128 threads on a shared /
-    cgroup-limited host is >10x slower than with 16-32 (measured r01), so the count is calibrated, then stated."""
+    cgroup-limited host can be many times slower than with 16-32, so the count is calibrated, then stated."""
     import torch
     from oracle import rife46 as O
     ncpu = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
@@ -141,8 +149,8 @@ def _pick_threads(sd):
 
 def bind_to_gpu_numa_node(local_rank):
     """Multi-process runs: pin this rank's threads (and, by first touch, its host buffers) to the NUMA node its GPU hangs
-    off.  r01: eight unbound ranks streaming pinned H2D + D2H at once reached 14.9 GB/s per direction per GPU against 41
-    alone (GPU0-3 sit on node 0, GPU4-7 on node 1).  Returns a description for the JSON line, or None."""
+    off: unbound ranks streaming pinned H2D + D2H at once share the remote socket's memory links.  Returns a description
+    for the JSON line, or None."""
     try:
         import torch
         pr = torch.cuda.get_device_properties(local_rank)
@@ -186,6 +194,24 @@ def cpu_port_fps(clip, sd, steps, warmup, min_seconds=0.0, keep=None):
     return n * len(times) / sum(times), sum(times) / len(times), threads, ncpu, len(times)
 
 
+def dump_outputs(out_dir, parts, sample=3_000_000, seed=20240611):
+    """The arrays a caller of the timed path receives (its interpolated frames), float32, < 64 MB at 1080p: the first and
+    the last frame whole (2 x 24.9 MB) and `sample` values of the whole output at seeded positions (12 MB).  `parts`: the
+    output as equally shaped [frames, H, W, 3] blocks in order (one per rank for N > 1), read in place."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    per = parts[0].numel()
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randint(0, per * len(parts), (min(sample, per * len(parts)),), generator=g).sort().values
+    vals = torch.empty(idx.numel(), dtype=torch.float32)
+    for r, p in enumerate(parts):
+        sel = (idx >= r * per) & (idx < (r + 1) * per)
+        vals[sel] = p.reshape(-1)[(idx[sel] - r * per).to(p.device)].float().cpu()
+    np.save(os.path.join(out_dir, "frames_first_last.npy"), torch.stack([parts[0][0], parts[-1][-1]]).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "frames_sample.npy"), vals.numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -201,7 +227,11 @@ def main():
                          "[4] through tools/bench_film.py / tools/bench_sepconv.py (same JSON-line contract, own metric name)")
     ap.add_argument("--arch", default="4.6", choices=["4.6", "4.7", "4.17", "4.26"],
                     help="RIFE arch (default 4.6 = the BASELINE.json metric; the others are side measurements)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's interpolated frames (a fixed, seeded sample of them) as .npy to DIR")
     a, extra = ap.parse_known_args()
+    if a.dump_outputs and (a.workload != "rife" or a.impl == "reference"):
+        ap.error("--dump-outputs writes the frames of the RIFE GPU path only (not with --impl reference or another --workload)")
     if a.workload != "rife":  # the other model families keep their own harness; same launch convention (torchrun for N > 1)
         import runpy
         tool = {"film": "bench_film.py", "sepconv": "bench_sepconv.py", "gmfss": "bench_gmfss.py"}[a.workload]
@@ -251,7 +281,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import __graft_entry__ as ge
     ge.load_package()
     from cfi_b200.engine import Rife46Engine
@@ -295,9 +325,9 @@ def main():
         eng.forward(dev_clip, f0[lo:hi], f1[lo:hi], ts[lo:hi], out=dev_out[lo:hi])
 
     # the only exchange of the path, inside the timed region for N > 1: every rank's interpolated frames end up on rank 0.
-    # Default: chunked dist.gather (NCCL send / recv kernels over NVLink, 595 GB/s alone at N = 2).  VFI_GATHER=push: copy-engine
-    # pushes into an IPC-shared buffer on rank 0 (shard.PushGather) - measured r02 on this pool: 35 GB/s, i.e. the IPC mapping
-    # gets no peer access inside these containers and the copy is staged through the host, so it stays an option only.
+    # Default: chunked dist.gather (NCCL send / recv kernels over NVLink).  VFI_GATHER=push: copy-engine pushes into an
+    # IPC-shared buffer on rank 0 (shard.PushGather) - an option only: where the IPC mapping gets no peer access (some
+    # containers) the copy is staged through the host.
     pusher = None
     if dist is not None and os.environ.get("VFI_GATHER", "nccl") == "push":
         pusher = shard.PushGather(npairs, (H, W, 3), torch.float32, dist, dst=0)
@@ -332,6 +362,11 @@ def main():
     t_end = time.time()
     launches = eng.launch_count() - l0
     ms_dev = e0.elapsed_time(e1)
+    if a.dump_outputs and rank == 0:  # what rank 0 holds after the step: its own frames, or every rank's as gathered there
+        if dist is None:
+            dump_outputs(a.dump_outputs, [dev_out])
+        else:
+            dump_outputs(a.dump_outputs, list(pusher.buffer) if pusher is not None else gather_list)
     clocks = sampler.stop(t_begin, t_end) if rank == 0 else None
     gather_ok = None
     if dist is not None:  # what landed on rank 0 is what every rank computed (sums of each rank's first and last frame)
@@ -343,7 +378,7 @@ def main():
             gather_ok = all(bool(torch.equal(torch.stack([got[r][0].double().sum(), got[r][-1].double().sum()]), sums[r]))
                             for r in range(world))
 
-    # ---- end to end through the bare C-ABI call on pre-pinned buffers ("e2e_capi", the r01 figure)
+    # ---- end to end through the bare C-ABI call on pre-pinned buffers ("e2e_capi")
     host_in = clip.contiguous().pin_memory()
     host_out = torch.empty((npairs, H, W, 3), dtype=torch.float32).pin_memory()
     for _ in range(max(1, min(a.warmup, 2))):
@@ -425,12 +460,8 @@ def main():
         k_ms = sum(tl) / len(tl)
         k_flops = 2.0 * pl["macs_per_cell"] * B * 272 * 480
         achieved = k_flops / (k_ms * 1e-3) / 1e12
-        roofline = {"kernel": "tapconv_kernel (block-3 ResConv 64->64, 272x480 cells, tcgen05)", "bound": "tensor",
+        roofline = {"kernel": "tapconv_kernel (block-3 ResConv 64->64, 272x480 cells, wgmma)", "bound": "tensor",
                     "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
-                    # dram__bytes_read.sum + dram__bytes_write.sum of this launch (batch 8) in the committed capture
-                    # profiles/r02_c_resconv_b3.ncu-rep: 133.8 MB + 90.6 MB against 2 x 133.7 MB of algorithmic
-                    # activation bytes (part of the output is still in L2 when the kernel ends); not re-measured here
-                    "traffic": (224.4e6 if B == 8 else None), "traffic_source": "ncu profiles/r02_c_resconv_b3 (133.8 MB read + 90.6 MB written)",
                     "algorithmic_bytes": 2.0 * B * 272 * 480 * 64 * 2,
                     "peak_source": peaks["source"] + ", burst figure (kernel timed alone)",
                     "launch_ms": k_ms, "flops_per_launch": k_flops}
@@ -447,26 +478,22 @@ def main():
             return prof[gid][0] / npairs if gid in prof else None
         hbm_rows = []
         if a.arch == "4.6":
-            # traffic: dram__bytes_read.sum + dram__bytes_write.sum of the same kernels in the committed capture
-            # profiles/r02_i_elementwise.ncu-rep (one pass of 8 pairs: 1497 / 1382 / 645 MB), per pair
-            for gid, name, bpp, traffic in (
-                    (30, "front<block 3> (flow up-sample + 2 warps + resample + concat -> conv0.0 input)", 16 + 20 + 20 + 5 + 32, 1497e6 / 8),
-                    (90, "final (flow up-sample + 2 warps + sigmoid blend + crop + clamp)", 20 + 20 + 32 + 12 * (H * W) / px, 1382e6 / 8),
-                    (20, "front<block 2> (same at scale 2; stores the accumulated flow plane)", 16 + 1.5625 + 32 / 4 + 20, 645e6 / 8)):
+            for gid, name, bpp in (
+                    (30, "front<block 3> (flow up-sample + 2 warps + resample + concat -> conv0.0 input)", 16 + 20 + 20 + 5 + 32),
+                    (90, "final (flow up-sample + 2 warps + sigmoid blend + crop + clamp)", 20 + 20 + 32 + 12 * (H * W) / px),
+                    (20, "front<block 2> (same at scale 2; stores the accumulated flow plane)", 16 + 1.5625 + 32 / 4 + 20)):
                 ms = per_pair_ms(gid)
                 if ms:
                     gbs = bpp * px / (ms * 1e-3) / 1e9
                     hbm_rows.append({"kernel": name, "ms_per_pair": ms, "bytes_per_pair": bpp * px, "achieved": gbs,
-                                     "frac": gbs / peaks["hbm_gbs"], "traffic": traffic if a.batch == 8 else None})
+                                     "frac": gbs / peaks["hbm_gbs"]})
         roofline_hbm = {"bound": "hbm", "unit": "GB/s", "peak": peaks["hbm_gbs"], "peak_source": peaks["source"],
                         "how": "CUDA events on the launching stream around each launch inside one profiled 63-pair step "
                                "(vfi_rife_profile); bytes = what the kernel must read + write per pair in this schedule",
                         "kernels": hbm_rows,
                         "achieved": hbm_rows[0]["achieved"] if hbm_rows else None,
                         "frac": hbm_rows[0]["frac"] if hbm_rows else None,
-                        "kernel": hbm_rows[0]["kernel"] if hbm_rows else None,
-                        "traffic": hbm_rows[0]["traffic"] if hbm_rows else None,
-                        "traffic_source": "ncu profiles/r02_i_elementwise.ncu-rep (per pair = per-launch bytes / 8)"}
+                        "kernel": hbm_rows[0]["kernel"] if hbm_rows else None}
         groups = {str(k): {"ms_per_pair": v[0] / npairs, "spans": v[1]} for k, v in sorted(prof.items())}
         del x, y, flush
 
@@ -487,7 +514,7 @@ def main():
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
                 "ms_per_step": ms_dev / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "bf16" if a.dtype == "bfloat16" else "f16",
-                "dtype_note": "conv operands 16-bit, fp32 accumulate (TMEM); flow/mask/warp/blend fp32; PSNR>=50 dB "
+                "dtype_note": "conv operands 16-bit, fp32 accumulate (registers); flow/mask/warp/blend fp32; PSNR>=50 dB "
                               "vs fp32 oracle enforced by tests/test_gpu_forward.py",
                 "data": "synthetic", "config": config,
                 "e2e": {"value": e2e, "unit": UNIT, "ms_per_step": ms_e2e / a.steps, "via": "RIFE_VFI.vfi (node call)",

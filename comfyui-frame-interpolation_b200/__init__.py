@@ -1,4 +1,4 @@
-"""B200-native drop-in for the RIFE (and FILM) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
+"""H100-native drop-in for the RIFE (and FILM) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
 
 Exports the same mapping names ComfyUI discovers in the reference's root __init__.py:23-47.
 """
@@ -17,8 +17,8 @@ NODE_CLASS_MAPPINGS = {
 }
 
 NODE_DISPLAY_NAME_MAPPINGS = {
-    "RIFE VFI": "RIFE VFI (B200 native, rife4.6)",
-    "FILM VFI": "FILM VFI (B200 native)",
-    "Sepconv VFI": "Sepconv VFI (B200 native)",
-    "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (B200 native, union)",
+    "RIFE VFI": "RIFE VFI (H100 native, rife4.6)",
+    "FILM VFI": "FILM VFI (H100 native)",
+    "Sepconv VFI": "Sepconv VFI (H100 native)",
+    "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native, union)",
 }

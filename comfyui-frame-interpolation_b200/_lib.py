@@ -32,7 +32,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise VfiError(
-            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for this path.")
     L = C.CDLL(LIB_PATH)
     vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float

@@ -1,4 +1,4 @@
-"""Compile libvfi_b200.so in-tree with nvcc for sm_100a (no other architecture, no JIT cache)."""
+"""Compile libvfi_b200.so in-tree with nvcc for sm_90a (no other architecture, no JIT cache)."""
 import os
 import shutil
 import subprocess
@@ -25,7 +25,7 @@ def needs_build():
 def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "--threads", "4", "-Xcompiler", "-fPIC,-mavx2", "-shared", "-o", LIB] + [os.path.join(CSRC, s) for s in SOURCES]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

@@ -113,9 +113,8 @@ __device__ __forceinline__ float4 sample_border4(const uint2* __restrict__ img, 
 //      flow(p) = base(p) + sum_j up(T_j)(p) * s_j          (same fp32 summation order as the reference)
 // where `base` is a full-resolution plane that is written only by a front kernel that visits every pixel anyway
 // (s <= 2), never by a separate pass: with scales 8,4,2,1  block 1 reads {T0}, block 2 reads {T0,T1} and stores
-// F1, block 3 reads F1+{T2} and stores F2, the final blend reads F2+{T3}.  (ncu r01: a fully implicit variant was
-// instruction bound - 24 extra loads per pixel in block 3 - and a separate up-sample/accumulate pass per block
-// moved 2x the bytes.)
+// F1, block 3 reads F1+{T2} and stores F2, the final blend reads F2+{T3}.  (A fully implicit variant needs 24 extra
+// loads per pixel in block 3, and a separate up-sample/accumulate pass per block moves 2x the bytes.)
 // ---------------------------------------------------------------------------------------------
 struct FlowLevels {
   const float4* f[kMaxBlocks];  // levels to add, in order: [B, Hp/s, Wp/s] flow increments
@@ -207,8 +206,7 @@ __global__ void front_kernel(const uint2* __restrict__ imgs, const FlowLevels le
   const int Hs = Hp / s, Ws = Wp / s;
   const size_t plane = (size_t)Hp * Wp;
   const float inv_s = 1.f / (float)s;
-  // grid = (x cells / 64, row pairs, images): no integer division per thread (ncu r01_v11: the 64-bit div/mod of a
-  // flat index was a large part of the ~450 instructions per pixel)
+  // grid = (x cells / 64, row pairs, images): no 64-bit integer division of a flat index per thread
   {
     const int par = (int)(threadIdx.x & 1);
     const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
@@ -490,8 +488,8 @@ __global__ void encode_deconv_kernel(const float* __restrict__ e16, const float*
         }
       }
     }
-    // half4: the features only ever feed the 16-bit block inputs (r01_v13: the 4.7 fronts were gather bound on 16-byte
-    // image and feature texels, 1453 frames/s against 2452 for arch 4.6)
+    // half4: the features only ever feed the 16-bit block inputs (the 4.7 fronts gather image and feature texels; 8 bytes
+    // each instead of 16)
     feats[id] = make_uint2(Pack2<__half>::pack(o[0], o[1]), Pack2<__half>::pack(o[2], o[3]));
   }
 }
@@ -1277,7 +1275,7 @@ __global__ void warp_kernel(const float* __restrict__ img, const float* __restri
 
 inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = 148 * 32;  // grid-stride loops: a few waves of the 148 SMs
+  const size_t cap = 132 * 32;  // grid-stride loops: a few waves of the 132 SMs
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 

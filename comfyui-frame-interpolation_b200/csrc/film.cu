@@ -1,4 +1,4 @@
-// FILM (film_net) on B200: weight repacking, workspace, the forward schedule and its C ABI (include/vfi_b200.h).
+// FILM (film_net) on H100: weight repacking, workspace, the forward schedule and its C ABI (include/vfi_b200.h).
 // SURVEY.md section 8 row a10.  Reference: vfi_models/film/film_arch.py, Interpolator.debug_forward :401-456.
 //
 // Forward schedule for B frame pairs (images are indexed k*B + pair, k = 0 first frame, 1 second frame; H_l = H >> l):

@@ -107,8 +107,7 @@ __global__ void conv2d_kernel(const float* __restrict__ in, const float* __restr
 // (output channel fastest, padded to a multiple of 16, gmfss.Ops.pack_conv) so that the 16 weights of a tap are four 16-byte
 // loads; thread = (n, 16 output channels, yo, PX = 8 consecutive xo); per (ci, ky) the input row segment the 8 pixels need
 // is loaded once into registers and reused by all kx taps: (7 S + K) + 4 K loads for 128 K multiply-adds, K and the stride S
-// compile-time so that everything stays in registers.  (First GPU run of the scalar-weight form above, r02: 4.7 TFLOP/s over
-// the whole GMFSS frame - one scalar weight load per four multiply-adds.)
+// compile-time so that everything stays in registers (the scalar-weight form above loads one weight per four multiply-adds).
 template <int K, int S>
 __global__ void conv2d_packed_kernel(const float* __restrict__ in, const float* __restrict__ wt, const float* __restrict__ bias,
                                      const float* __restrict__ res1, const float* __restrict__ res2, float* __restrict__ out, int N,
@@ -815,8 +814,8 @@ cudaError_t gm_gemm(int bt, const float* A, const float* B, const float* bias, c
   const bool aligned = ((K | N | lda | ldb) & 3) == 0 && (N & 7) == 0 && ((sA | sB) & 3) == 0 &&
                        ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15) == 0;
   if (!bt && aligned) {
-    // rows per thread: 8 when that still gives the GPU enough threads, else 4 or 2 (r02 capture: the 7680 x 128 x 1024 linear
-    // ran as 120 blocks of 8 x 8-tile threads - 6 % of the warp slots - and took 456 us)
+    // rows per thread: 8 when that still gives the GPU enough threads, else 4 or 2 (a 7680 x 128 x 1024 linear with 8 rows
+    // per thread is only 120 blocks of 8 x 8-tile threads)
     const size_t cols = (size_t)nb * (N / 8);
     const int mt = cols * ((M + 7) / 8) >= 60000 ? 8 : (cols * ((M + 3) / 4) >= 60000 ? 4 : 2);
     const size_t threads = cols * ((M + mt - 1) / mt);

@@ -24,8 +24,7 @@ namespace vfi {
 // the CPU again, so the lines are written without first being fetched (no read-for-ownership: a third less DRAM
 // traffic than a cached copy) and without evicting the source stream from the cache.  Falls back to memcpy for small or
 // unaligned-tail pieces and when the translation unit is built without AVX2.
-inline bool use_stream_stores() {  // VFI_NT_COPY=0: plain memcpy (A/B runs).  r02 on the B200 host (Xeon 8562Y+, 12 copy
-  // threads, NUMA-local): node e2e 1143 frames/s with memcpy, 1300 with the streaming stores (profiles/r02_f_*)
+inline bool use_stream_stores() {  // VFI_NT_COPY=0: plain memcpy (A/B runs)
   static const bool on = [] {
     const char* e = std::getenv("VFI_NT_COPY");
     return !(e && e[0] == '0');

@@ -1,5 +1,5 @@
 // The reference's custom CUDA ops (vfi_models/ops/cupy_ops, CUDA-C strings JIT-compiled through cupy/NVRTC), rebuilt as
-// ahead-of-time sm_100a kernels behind the C ABI.  Same tensor contract as the reference: contiguous NCHW fp32.
+// ahead-of-time sm_90a kernels behind the C ABI.  Same tensor contract as the reference: contiguous NCHW fp32.
 //   softsplat_sum  : forward summation splat                      cupy_ops/softsplat.py:140-192
 //   costvol_l1     : 9x9 L1 cost volume (81 ch)                   cupy_ops/costvol.py:4-43
 //   corr_dot       : 9x9 dot-product correlation (81 ch)          cupy_ops/correlation.py:4-99
@@ -237,9 +237,9 @@ __global__ void __launch_bounds__(256) volume81_tile_kernel(const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
-// Channel-last forms (r02).  The reference's tensors are NCHW, and both ops above pay for it: the splat issues four scalar
-// atomics per (pixel, channel) into four different planes (r01 / r02 measurements: 4 - 14 % of HBM bandwidth), the volumes
-// read one value per (channel, displacement) from shared memory (one LDS per multiply-add, 6.7 % of the fp32 rate).  With
+// Channel-last forms.  The reference's tensors are NCHW, and both ops above pay for it: the splat issues four scalar
+// atomics per (pixel, channel) into four different planes, the volumes read one value per (channel, displacement) from
+// shared memory (one LDS per multiply-add).  With
 // the channels of a pixel contiguous, a splat corner is ONE 16-byte vector atomic per four channels and a displacement of
 // the volume is a dot product of two contiguous channel vectors, reduced over the lanes of a warp with shuffles.  The C-ABI
 // keeps the reference's NCHW contract: the inputs are transposed into context-owned scratch first (coalesced both ways),
@@ -461,7 +461,7 @@ __global__ void __launch_bounds__(256) sepconv_tile_kernel(const float* __restri
 
 inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 

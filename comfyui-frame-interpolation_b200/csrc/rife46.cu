@@ -56,7 +56,7 @@ uint16_t to_operand(float v, int op_type) {
   return u;
 }
 
-// Packed weights = the SWIZZLE_128B K-major UMMA B operand, bit for bit: [split][K16/4 (padded)][n][128-byte row of
+// Packed weights = the SWIZZLE_128B K-major wgmma B operand, bit for bit: [split][K16/4 (padded)][n][128-byte row of
 // four K=16 steps], 16-byte chunks XOR-swizzled with (n & 7); bulk-copied to shared memory verbatim.
 template <class F>
 std::vector<uint16_t> pack_weights(const TapConvLayer& L, int op_type, F wfun) {
@@ -103,30 +103,6 @@ void choose_split(TapConvLayer& L, const std::vector<int>& splits, int want_stag
   L.n_cta = L.n_total / best_split;
 }
 
-// CTA-pair form (tapconv.cu, cta_group::2): pair-split s covers n_epi = n_total / psp output channels, each CTA of the
-// pair holding half of them as its B rows (packed slices 2s and 2s+1).  Returns false when no split reaches
-// `want_stages` (the caller then keeps the single-CTA plan).  VFI_PAIR=0 switches the form off (A/B runs).
-bool choose_split_pair(TapConvLayer& L, const std::vector<int>& psplits, int want_stages) {
-  static const bool on = [] {
-    const char* e = std::getenv("VFI_PAIR");
-    return !(e && e[0] == '0');
-  }();
-  if (!on) return false;
-  const TapConvLayer keep = L;
-  for (int psp : psplits) {
-    if (L.n_total % (2 * psp)) continue;
-    const int n_epi = L.n_total / psp;
-    if ((n_epi & 15) || n_epi > 128) continue;
-    L.pair = 1;
-    L.nsplit = 2 * psp;
-    L.n_cta = n_epi / 2;
-    TapConvParams p{};
-    if (tapconv_plan(L, &p) >= want_stages) return true;
-  }
-  L = keep;
-  return false;
-}
-
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
@@ -153,7 +129,7 @@ using namespace vfi;
 
 struct vfi_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   int batch = 8;
   int op_type = OP_F16;
   bool loaded = false;
@@ -281,9 +257,9 @@ void set_taps_3x3(TapConvLayer& L, int ch, bool ring) {
 }
 
 // Wide, deep layers (c = 128, 192): with the whole window staged per tile the resident weight slice leaves room for
-// only n_cta = 16..32 output channels, and one tcgen05.mma costs ~80 cycles whatever its N (profiles/README.md), so
-// the layer time is ~ 1/n_cta.  The ring pipeline stages one 64-channel k-block at a time, which frees shared
-// memory for n_cta = 48 (c = 192) / 64 (c = 128).  VFI_RING=0 disables it (A/B runs).
+// only n_cta = 16 output channels, and every wgmma reads its whole 64-row A block from shared memory whatever its N, so
+// narrow CTAs re-read the window once per split.  The ring pipeline stages one 64-channel k-block at a time, which
+// frees shared memory for n_cta = 32 (c = 192) / 64 (c = 128).  VFI_RING=0 disables it (A/B runs).
 bool want_ring(int ch) {
   static const bool on = [] {
     const char* e = std::getenv("VFI_RING");
@@ -302,12 +278,7 @@ int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const 
   L.epi_mode = EPI_RESCONV;
   const bool ring = want_ring(ch);
   set_taps_3x3(L, ch, ring);
-  // CTA pairs where they halve the output-channel splits (c >= 96).  Measured at the 1080p geometry, batch 8
-  // (profiles/r02_b_layers_b8_{pair,nopair}.json): c = 96 60.4 -> 46.1 us, c = 128 33.8 -> 31.7, c = 192 29.7 -> 25.6; at
-  // c = 64, where a single CTA already holds all 64 columns, the pair is SLOWER (82.9 -> 91.2 us: half of every MMA's B
-  // operand then comes from the peer SM's shared memory), so the 64-channel layers stay single-CTA.
-  if (!(ch >= 96 && choose_split_pair(L, {1, 2, 3, 4, 6}, ring ? 2 : 3)))
-    choose_split(L, {1, 2, 3, 4, 6, 8, 12}, ring ? 2 : 3);
+  choose_split(L, {1, 2, 3, 4, 6, 8, 12}, ring ? 2 : 3);
   // (conv(x) + b) * beta + x  ==  conv_{w*beta}(x) + b*beta + x : beta is folded into the packed weights (one 16-bit
   // rounding of w*beta instead of w) so the epilogue is a pure add
   auto wf = [&](int e, int ci, int n) -> float {  // e = kb * 9 + tap (kb = 0 unless ring), ci relative to the k-block
@@ -336,14 +307,10 @@ int build_lastconv(vfi_ctx* c, TapConvLayer& L, int ch, int cout, const float* w
   L.epi_mode = EPI_LASTCONV;
   const bool ring = want_ring(ch);
   set_taps_3x3(L, ch, ring);
-  // all 80 columns in one CTA pair (40 B rows each) only where single CTAs would need five splits (c = 192: 27.6 ->
-  // 19.5 us); elsewhere the single-CTA form is as fast or faster (c = 64: 93.2 vs 111.6 us, same measurement as above)
-  if (!(ch >= 192 && choose_split_pair(L, {1}, 2))) {
+  choose_split(L, {1, 5}, 2);
+  if (ring && L.nsplit != 1) {  // the ring only pays when it keeps all 80 columns in one CTA (c = 128)
+    set_taps_3x3(L, ch, false);
     choose_split(L, {1, 5}, 2);
-    if (ring && L.nsplit != 1) {  // the ring only pays when it keeps all 80 columns in one CTA (c = 128)
-      set_taps_3x3(L, ch, false);
-      choose_split(L, {1, 5}, 2);
-    }
   }
   auto oc_of = [](int n) {
     const int c5 = n >> 4, pos = n & 15, py = pos >> 2, px = pos & 3;
@@ -589,9 +556,8 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
     if (c->profile) cudaEventRecord(c->prof_spans.back().e1, st);
   };
   // The last block's front stores the accumulated flow too and `final` adds one level to it.  VFI_FLOW_STORE_LAST=0: it
-  // does not, `final` adds the last TWO levels on the fly.  Measured r02 (profiles/r02_c_bench*.log, per pair): the
-  // largest front 38.1 -> 33.6 us without its 20 B/px store, but `final` 35.8 -> 45.4 us (the second level's eight taps
-  // per pixel make it instruction bound) - a net loss, so storing stays the default.
+  // does not, `final` adds the last TWO levels on the fly: the largest front then saves its 20 B/px store, but `final`
+  // reads a second level with eight taps per pixel, which makes it instruction bound - so storing stays the default.
   static const bool store_last = [] {
     const char* e = std::getenv("VFI_FLOW_STORE_LAST");
     return !(e && e[0] == '0');
@@ -681,7 +647,7 @@ int check_tasks(const int32_t* f0, const int32_t* f1, int n_tasks, int lo, int h
 extern "C" {
 
 const char* vfi_last_error(void) { return g_err.c_str(); }
-const char* vfi_version(void) { return "vfi_b200 0.2 (sm_100a; RIFE 4.6/4.7/4.17/4.26, FILM, Sepconv, GMFSS Fortuna building blocks; built " __DATE__ " " __TIME__ ")"; }
+const char* vfi_version(void) { return "vfi_b200 0.3 (sm_90a; RIFE 4.6/4.7/4.17/4.26, FILM, Sepconv, GMFSS Fortuna building blocks; built " __DATE__ " " __TIME__ ")"; }
 
 int vfi_create(int device, vfi_ctx** out) {
   if (!out) return fail(VFI_E_INVALID, "null out");
@@ -691,7 +657,7 @@ int vfi_create(int device, vfi_ctx** out) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(VFI_E_INVALID, "libvfi_b200 needs a compute-capability 10.x (B200, sm_100a) GPU");
+  if (prop.major != 9) return fail(VFI_E_INVALID, "libvfi_b200 needs a compute-capability 9.x (H100, sm_90a) GPU");
   vfi_ctx* c = new vfi_ctx();
   c->device = device;
   c->num_sms = prop.multiProcessorCount;
@@ -955,7 +921,7 @@ int vfi_rife46_interpolate_host(vfi_ctx* c, const float* frames, int n_frames, i
   const size_t frame_bytes = frame_elems * sizeof(float), out_bytes = out_elems * sizeof(float);
   // pass sizes: full batches in the middle; on a long clip the first and the last passes are small (1, 2, 4 pairs) so
   // that the exposed head (upload before the first pass) and tail (download after the last) are one or two frames
-  // instead of a whole batch (r01: 64 frames e2e = 63 x 0.574 ms + 7.3 ms of head and tail with uniform passes)
+  // instead of a whole batch
   std::vector<int> pass_pos, pass_n;
   {
     const bool ramp = B >= 8 && n_tasks >= 4 * B;
@@ -981,8 +947,8 @@ int vfi_rife46_interpolate_host(vfi_ctx* c, const float* frames, int n_frames, i
   // ---- the prepared-frame window is a RING: only frames some task references are uploaded, in order of first use, into
   // slot (upload counter % R).  R covers every frame from its upload to the pass after its last use, so that the slot a
   // pass's uploads overwrite was last read two passes ago (the copy stream runs one pass ahead of the compute stream
-  // without waiting) - 2 B + 1 slots for consecutive pairs instead of the whole clip (r01: 50-67 MB per 1080p frame for
-  // every frame of the clip; a few thousand frames did not fit).  An event wait keeps any reuse correct regardless.
+  // without waiting) - 2 B + 1 slots for consecutive pairs instead of the whole clip (tens of MB per 1080p frame: a clip
+  // of a few thousand frames would not fit).  An event wait keeps any reuse correct regardless.
   std::vector<int> first_pass(nf, -1), last_pass(nf, -1), ctr(nf, -1), up_frames, up_end(nb, 0);
   for (int k = 0; k < nb; ++k)
     for (int i = 0; i < pass_n[k]; ++i)
@@ -1015,9 +981,8 @@ int vfi_rife46_interpolate_host(vfi_ctx* c, const float* frames, int n_frames, i
   // the H2D copies, a downloader thread empties the D2H ring into the caller's tensor; each uses a few copy threads.
   // Pass-through frames (frame_slot): source frame f is also wanted unchanged (first 3 channels) at out + frame_slot[f].
   // The uploader thread makes that copy - and when `out` is page-locked the frame is then UPLOADED FROM THERE: the one
-  // host copy the node contract needs anyway doubles as the staging copy (r02: staging and pass-through as two separate
-  // copies ran at ~20 GB/s each on the box's cgroup-limited host cores and were the critical path, 91 ms for a 40 ms
-  // pipeline).
+  // host copy the node contract needs anyway doubles as the staging copy (staging and pass-through as two separate host
+  // copies can become the critical path on a few host cores).
   const bool stage_out = !is_pinned_host(out);
   auto via_out = [&](int f_abs) { return frame_slot != nullptr && !stage_out && frame_slot[f_abs] >= 0; };
   bool any_ring = false, any_pt = false;
@@ -1347,10 +1312,9 @@ int vfi_costvol_l1(vfi_ctx* c, const float* one, const float* two, float* out, i
                    void* stream) {
   if (!c || !one || !two || !out || N < 1 || C < 1 || H < 1 || W < 1) return fail(VFI_E_INVALID, "bad argument");
   CK(cudaSetDevice(c->device));
-  // VFI_VOLUME_WARP=1: the warp-per-pixel channel-last form (shuffle reduction over the channels).  Measured r02
-  // (profiles/r02_h_bench_ops*.log): 189 / 705 us against 123 / 258 us of the shared-memory tiled kernel on the 64-channel
-  // 96x160 and 128-channel 192x320 shapes - each displacement re-reads its channel vector through L1, 81 times per pixel -
-  // so the tiled kernel stays the default and this form is kept for comparison.
+  // VFI_VOLUME_WARP=1: the warp-per-pixel channel-last form (shuffle reduction over the channels).  Each displacement
+  // re-reads its channel vector through L1, 81 times per pixel, so the shared-memory tiled kernel stays the default and
+  // this form is kept for comparison.
   static const bool warp_form = [] {
     const char* e = std::getenv("VFI_VOLUME_WARP");
     return e && e[0] == '1';
@@ -1371,10 +1335,9 @@ int vfi_corr_dot(vfi_ctx* c, const float* first, const float* second, float* out
                  void* stream) {
   if (!c || !first || !second || !out || N < 1 || C < 1 || H < 1 || W < 1) return fail(VFI_E_INVALID, "bad argument");
   CK(cudaSetDevice(c->device));
-  // VFI_VOLUME_WARP=1: the warp-per-pixel channel-last form (shuffle reduction over the channels).  Measured r02
-  // (profiles/r02_h_bench_ops*.log): 189 / 705 us against 123 / 258 us of the shared-memory tiled kernel on the 64-channel
-  // 96x160 and 128-channel 192x320 shapes - each displacement re-reads its channel vector through L1, 81 times per pixel -
-  // so the tiled kernel stays the default and this form is kept for comparison.
+  // VFI_VOLUME_WARP=1: the warp-per-pixel channel-last form (shuffle reduction over the channels).  Each displacement
+  // re-reads its channel vector through L1, 81 times per pixel, so the shared-memory tiled kernel stays the default and
+  // this form is kept for comparison.
   static const bool warp_form = [] {
     const char* e = std::getenv("VFI_VOLUME_WARP");
     return e && e[0] == '1';

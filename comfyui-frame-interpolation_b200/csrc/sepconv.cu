@@ -1,4 +1,4 @@
-// Sepconv ("revisiting adaptive convolutions", the reference's `Sepconv VFI` node) on B200: weights, workspace, forward
+// Sepconv ("revisiting adaptive convolutions", the reference's `Sepconv VFI` node) on H100: weights, workspace, forward
 // schedule and C ABI.  SURVEY.md section 8 row a12.  Reference: vfi_models/sepconv/sepconv_enhanced.py, Network :536-706.
 //
 // Forward for B pairs (levels: row 0 = He x We (input padded to even), row r = ceil(row r-1 / 2); C_r = 32,64,128,256,512):

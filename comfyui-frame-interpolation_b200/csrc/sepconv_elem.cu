@@ -249,8 +249,7 @@ __global__ void add_crop16_kernel(const T* __restrict__ v, int Hv, int Wv, T* __
 
 // [B, HW, pitch] 16-bit (pitch = 64: the head's padded channel count) -> [B, K, HW] fp32.  Tiles of 32 pixels through shared
 // memory so that both sides are coalesced: a pixel's channels are read as 32-bit words (128 B per pixel), a channel's 32 pixels
-// are written as 128 B.  (r02 launch list: the first version - one thread per output element reading a 2-byte value with a
-// 128-byte stride - took 1.94 ms per launch at 1080p, 48 % of a Sepconv frame; 636 MB of traffic is ~0.1 ms of HBM time.)
+// are written as 128 B (one thread per output element would read a 2-byte value with a 128-byte stride).
 // Written for any blockDim (the host emulation runs it with one thread per block).
 template <typename T>
 __global__ void sep_coeff_nchw_kernel(const T* __restrict__ in, int pitch, float* __restrict__ out, int K, int B, size_t hw) {

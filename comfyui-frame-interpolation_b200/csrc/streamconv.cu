@@ -1,5 +1,5 @@
-// streamconv: implicit-GEMM convolution with STREAMED weights on the 5th-gen tensor cores (tcgen05 / TMEM / TMA),
-// sm_100a only.  The conv kernel of the FILM path (SURVEY.md section 8 row a10).
+// streamconv: implicit-GEMM convolution with STREAMED weights on the Hopper tensor cores (wgmma / TMA / mbarrier),
+// sm_90a only.  The conv kernel of the FILM path (SURVEY.md section 8 row a10).
 //
 // Replaces the cuDNN / ATen kernels behind film_arch.conv (film_arch.py:784-798: Conv2d(k x k, padding='same')
 // [+ LeakyReLU(0.2)], k = 1, 2, 3) for every layer of
@@ -11,28 +11,25 @@
 //   A  the input window of a tile (tile + halo) for ONE 64-channel k-block, dropped into shared memory by TMA as rows of
 //      128 B (SWIZZLE_128B) - exactly tapconv's ring slot: every filter tap is a descriptor START ADDRESS into the
 //      window ((dy*halo_w + dx) * 128 B, 8-row-group stride SBO = halo_w * 128 B), a K=16 step a 32-byte shift.  One CTA
-//      pass covers `mt` (1 or 2) tiles of 16 x 8 output pixels = mt accumulators of M = 128 rows, so a weight slice read
-//      from L2 feeds 2 x 128 rows;
+//      pass covers mt = 2 tiles of 16 x 8 output pixels, one per MMA warpgroup, so a weight slice read from L2 feeds
+//      2 x 128 rows;
 //   B  the weights of one (k-block, tap): [n_cta rows][64 channels = 128 B, 16-byte chunks XOR (n & 7)] = the
 //      SWIZZLE_128B K-major B operand bit for bit, packed that way on the host, one cp.async.bulk per slot.
 // A layer may read its input channels from TWO tensors (k-blocks [0, nkb0) from source 0, the rest from source 1):
 // torch.cat along channels (film_arch.py:541, :292, :781) never materialises.  Channel counts are padded to multiples of
 // 64 in HBM (zero weights for the padding), outputs go to any channel slice of a wider NHWC tensor.
 //
-// Warp roles (608 threads, 1 persistent CTA per SM):
-//   warps 0..15 : epilogue, four groups of four warps (TMEM lane quarters); group g < mt * nsets owns accumulator
-//                 (set g / mt, tile g % mt): tcgen05.ld -> + bias -> LeakyReLU / identity -> 16-bit -> 32-byte stores
-//   warp 16     : TMEM alloc / dealloc; one elected lane issues tcgen05.mma + tcgen05.commit
-//   warp 17     : one elected lane: A producer (one 4-D TMA per tile and k-block)
-//   warp 18     : one elected lane: B producer (one bulk copy per (k-block, tap))
-// Pipelines: A ring (2-4 slots, full = TMA bytes, empty = tcgen05.commit after the k-block's last tap), B ring (3-8
-// slots, full = bulk-copy bytes, empty = tcgen05.commit after the tap's MMAs), accumulator sets (full = commit after the
-// last k-block, empty = the set's epilogue warps).  Every wait is bounded (ptx.cuh mbar_wait) and traps.
-//
-// Round-1 status: first GPU run parity-green (profiles/r01_film_gpu_check.jsonl: tcgen05 vs the CUDA-core checker below
-// <= 6e-4 relative on 11 layer shapes, whole FILM net 64.4 dB vs the unmodified reference); not yet timed or profiled.
+// Warp roles (320 threads, 1 persistent CTA per SM):
+//   warpgroups 0, 1 : warpgroup t multiplies tile t of the pass (two m64 row blocks, accumulators in registers) and
+//                     runs its epilogue: + bias -> LeakyReLU / identity (ext: PReLU, + residual) -> 16-bit -> stores
+//   warp 8          : one elected lane: A producer (one 4-D TMA per tile and k-block)
+//   warp 9          : one elected lane: B producer (one bulk copy per (k-block, tap))
+// Pipelines: A ring (2-4 slots, full = TMA bytes, empty = both warpgroups after the k-block's last tap), B ring (3-8
+// slots, full = bulk-copy bytes, empty = both warpgroups after the tap's MMAs have completed).  Every wait is bounded
+// (ptx.cuh mbar_wait) and traps.
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "ptx.cuh"
 #include "vfi_internal.h"
@@ -41,19 +38,18 @@ namespace vfi {
 
 namespace {
 
-constexpr int kMaxASlots = 4, kMaxBSlots = 8, kMaxSets = 2;
+constexpr int kMaxASlots = 4, kMaxBSlots = 8;
 struct SCtrl {
   uint64_t a_full[kMaxASlots];
   uint64_t a_empty[kMaxASlots];
   uint64_t b_full[kMaxBSlots];
   uint64_t b_empty[kMaxBSlots];
-  uint64_t t_full[kMaxSets];
-  uint64_t t_empty[kMaxSets];
-  uint32_t tmem_base;
 };
 constexpr uint32_t kSCtrlBytes = 256;
 static_assert(sizeof(SCtrl) <= kSCtrlBytes, "control block");
-constexpr int kSEpiWarps = 16, kSMmaWarp = 16, kSAWarp = 17, kSBWarp = 18, kSThreads = 32 * 19;
+constexpr int kSMmaGroups = 2, kSAWarp = 8, kSBWarp = 9, kSThreads = 128 * kSMmaGroups + 64;
+// every warp of both MMA warpgroups arrives on an `empty` barrier once it has waited for the MMAs that read the slot
+constexpr uint32_t kSConsumerArrivals = 4 * kSMmaGroups;
 
 struct TileCoord {
   int b, ty, tx;
@@ -82,128 +78,51 @@ __device__ __forceinline__ void ring_next(uint32_t& slot, uint32_t& ph, uint32_t
   }
 }
 
-#ifndef VFI_HOST_EMU  // (tests/host_emu runs the schedule on the CPU with the checker kernel below; no tcgen05 there)
-// EXT = false is the FILM kernel as verified in r01 (bias + LeakyReLU(0.2) / identity).  EXT = true adds what the Sepconv
-// trunk needs in the epilogue: a PReLU with one learned slope (a > 0 ? a : slope * a, any sign / size of slope) and a
-// residual tensor added after it (same layout as the output; it may BE the output: every thread reads its 16 channels
-// before it writes them).
-//
-// CL = 2 (VFI_SC_CLUSTER=2; written at the end of r01, NEVER RUN, default off): two CTAs of a thread-block cluster work on
-// neighbouring passes of the same output-channel split and share every weight slot - each CTA's B producer fetches HALF of
-// a slot from L2 and the bulk copy is multicast into both CTAs' shared memory (each CTA's own `full` barrier counts the
-// bytes landing in it), and a slot's `empty` barrier (count 2) receives the multicast tcgen05.commit of BOTH CTAs' MMAs.
-// Weight bytes per SM and cycle halve (64 / (2 mt) B/clk), which is what the L2-bound estimate of DESIGN.md 6.1 asks for.
-template <typename T, bool EXT, int CL>
+#ifndef VFI_HOST_EMU  // (tests/host_emu runs the schedule on the CPU with the checker kernel below; no wgmma there)
+// EXT = false is the FILM kernel (bias + LeakyReLU(0.2) / identity).  EXT = true adds what the Sepconv trunk needs in
+// the epilogue: a PReLU with one learned slope (a > 0 ? a : slope * a, any sign / size of slope) and a residual tensor
+// added after it (same layout as the output; it may BE the output: every thread reads its two channels before it
+// writes them).
+template <typename T, bool EXT, int N>
 __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_constant__ StreamConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  SCtrl* ctrl = reinterpret_cast<SCtrl*>(smem);
   asm volatile("griddepcontrol.launch_dependents;");  // see tapconv.cu: programmatic dependent launch
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   // the k-th pass of this CTA is pass0 + k * pass_stride; passes past the end have no valid tile (zero-filled A, no stores)
-  int split, pass0, pass_stride, my_passes;
-  uint32_t crank = 0;
-  if constexpr (CL == 2) {
-    crank = cluster_ctarank();
-    const int pair = blockIdx.x >> 1;          // cluster index; p.ctas_per_split counts CLUSTERS per split here
-    split = pair % p.nsplit;
-    const int pf = pair / p.nsplit;
-    const int npp = (p.npasses + 1) >> 1;      // pass pairs
-    my_passes = (npp - pf + p.ctas_per_split - 1) / p.ctas_per_split;   // the same for both CTAs of the cluster
-    pass0 = 2 * pf + (int)crank;
-    pass_stride = 2 * p.ctas_per_split;
-  } else {
-    split = blockIdx.x % p.nsplit;
-    const int first = blockIdx.x / p.nsplit;
-    if (first >= p.ctas_per_split) return;
-    my_passes = (p.npasses - first + p.ctas_per_split - 1) / p.ctas_per_split;
-    pass0 = first;
-    pass_stride = p.ctas_per_split;
-  }
-  const int mt = p.mt, nsets = p.nsets;
+  const int split = blockIdx.x % p.nsplit;
+  const int first = blockIdx.x / p.nsplit;
+  if (first >= p.ctas_per_split) return;
+  const int my_passes = (p.npasses - first + p.ctas_per_split - 1) / p.ctas_per_split;
+  const int pass0 = first;
+  const int pass_stride = p.ctas_per_split;
+  const int mt = p.mt;
 
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_afull = smem_base + offsetof(SCtrl, a_full);
   const uint32_t bar_aempty = smem_base + offsetof(SCtrl, a_empty);
   const uint32_t bar_bfull = smem_base + offsetof(SCtrl, b_full);
   const uint32_t bar_bempty = smem_base + offsetof(SCtrl, b_empty);
-  const uint32_t bar_tfull = smem_base + offsetof(SCtrl, t_full);
-  const uint32_t bar_tempty = smem_base + offsetof(SCtrl, t_empty);
   const uint32_t a_smem = smem_base + p.off_a;
   const uint32_t b_smem = smem_base + p.off_b;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.a_slots; ++s) {
-      mbar_init(bar_afull + 8 * s, 1);   // producer's arrive.expect_tx (+ TMA bytes)
-      mbar_init(bar_aempty + 8 * s, 1);  // tcgen05.commit
+      mbar_init(bar_afull + 8 * s, 1);  // producer's arrive.expect_tx (+ TMA bytes)
+      mbar_init(bar_aempty + 8 * s, kSConsumerArrivals);
     }
     for (int s = 0; s < p.b_slots; ++s) {
       mbar_init(bar_bfull + 8 * s, 1);
-      mbar_init(bar_bempty + 8 * s, (uint32_t)CL);  // the tcgen05.commit of every CTA that reads the slot
-    }
-    for (int s = 0; s < nsets; ++s) {
-      mbar_init(bar_tfull + 8 * s, 1);                     // tcgen05.commit after the last k-block
-      mbar_init(bar_tempty + 8 * s, (uint32_t)(4 * mt));  // the 4 warps of each of the set's mt epilogue groups
+      mbar_init(bar_bempty + 8 * s, kSConsumerArrivals);
     }
     mbar_fence_init();
   }
-  if (warp == kSMmaWarp) tmem_alloc(smem_base + offsetof(SCtrl, tmem_base), p.tmem_cols);
-  tc_fence_before();
-  if constexpr (CL == 2)
-    cluster_sync_all();  // the peer's barriers are initialised before anything is multicast to them
-  else
-    __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
+  __syncthreads();
 
-  if (warp == kSMmaWarp) {
-    // ======================================================= MMA issuer (one lane)
-    if (elect_one_sync()) {
-      const uint32_t idesc = p.idesc;
-      const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);              // LBO(=1) | start address, 16-byte units
-      const uint32_t b_lo0 = (1u << 16) | (b_smem >> 4);
-      const uint32_t b_hi = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO = 8 rows x 128 B | version | SWIZZLE_128B
-      const uint32_t a_hi = p.a_hi;                                   // SBO = halo_w x 128 B | version | SWIZZLE_128B
-      const uint32_t a_slot_u = p.a_slot_bytes >> 4, a_win_u = p.a_win_bytes >> 4, b_slot_u = p.b_slot_bytes >> 4;
-      uint32_t aslot = 0, aph = 0, bslot = 0, bph = 0;
-      for (int k = 0; k < my_passes; ++k) {
-        const uint32_t set = (uint32_t)(k % nsets), use = (uint32_t)(k / nsets);
-        mbar_wait(bar_tempty + 8 * set, (use & 1u) ^ 1u, 12);
-        uint32_t accum = 0;
-        for (int kb = 0; kb < p.nkb; ++kb) {
-          mbar_wait(bar_afull + 8 * aslot, aph, 13);
-          for (int tap = 0; tap < p.ntaps; ++tap) {
-            mbar_wait(bar_bfull + 8 * bslot, bph, 14);
-            tc_fence_after();
-            const uint32_t b_lo = b_lo0 + bslot * b_slot_u;
-            for (int t = 0; t < mt; ++t) {
-              const uint32_t d_tmem = tmem_base + (set * (uint32_t)mt + (uint32_t)t) * p.acc_stride;
-              uint64_t a64 = ((uint64_t)a_hi << 32) | (uint64_t)(a_lo0 + aslot * a_slot_u + (uint32_t)t * a_win_u + p.tap_off[tap]);
-              uint64_t b64 = ((uint64_t)b_hi << 32) | (uint64_t)b_lo;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {  // 64 channels = four K=16 steps, +32 B each
-                umma_f16(d_tmem, a64, b64, idesc, (i == 0) ? accum : 1u);
-                a64 += 2;
-                b64 += 2;
-              }
-            }
-            accum = 1u;
-            if constexpr (CL == 2)
-              umma_commit_multicast(bar_bempty + 8 * bslot, (uint16_t)0x3);  // ... in both CTAs of the cluster
-            else
-              umma_commit(bar_bempty + 8 * bslot);  // weight slot free once these MMAs have read it
-            ring_next(bslot, bph, (uint32_t)p.b_slots);
-          }
-          umma_commit(bar_aempty + 8 * aslot);  // window slot free
-          ring_next(aslot, aph, (uint32_t)p.a_slots);
-        }
-        umma_commit(bar_tfull + 8 * set);  // accumulators of this pass complete
-      }
-    }
-  } else if (warp == kSAWarp) {
+  if (warp == kSAWarp) {
     // ======================================================= A producer
-    if (elect_one_sync()) {
+    if (lane == 0) {
       asm volatile("griddepcontrol.wait;" ::: "memory");  // the input is the previous kernels' output
       uint32_t slot = 0, ph = 0;
       for (int k = 0; k < my_passes; ++k) {
@@ -212,7 +131,7 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
         tc[0] = tile_coord(p, pass * mt);
         tc[1] = tile_coord(p, pass * mt + 1);
         for (int kb = 0; kb < p.nkb; ++kb) {
-          mbar_wait(bar_aempty + 8 * slot, ph ^ 1u, 15);
+          mbar_wait(bar_aempty + 8 * slot, ph ^ 1u);
           mbar_arrive_expect_tx(bar_afull + 8 * slot, (uint32_t)mt * p.a_tx_bytes);
           const bool s0 = kb < p.nkb0;
           const void* tm = s0 ? &p.tm[0] : &p.tm[1];
@@ -224,114 +143,123 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
         }
       }
     }
-    __syncwarp();
-  } else if (warp == kSBWarp) {
+    return;
+  }
+  if (warp == kSBWarp) {
     // ======================================================= B producer (weights never depend on a previous kernel)
-    if (elect_one_sync()) {
+    if (lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_split_bytes;
       uint32_t slot = 0, ph = 0;
       const int per_pass = p.nkb * p.ntaps;
       for (int k = 0; k < my_passes; ++k) {
         for (int j = 0; j < per_pass; ++j) {
-          mbar_wait(bar_bempty + 8 * slot, ph ^ 1u, 16);
-          mbar_arrive_expect_tx(bar_bfull + 8 * slot, p.b_slot_bytes);  // CL = 2: my half + the peer's half land here
-          if constexpr (CL == 2) {
-            const uint32_t half = p.b_slot_bytes >> 1;
-            bulk_g2s_multicast(b_smem + slot * p.b_slot_bytes + crank * half, wsrc + (size_t)j * p.b_slot_bytes + crank * half,
-                               half, bar_bfull + 8 * slot, (uint16_t)0x3);
-          } else {
-            bulk_g2s(b_smem + slot * p.b_slot_bytes, wsrc + (size_t)j * p.b_slot_bytes, p.b_slot_bytes, bar_bfull + 8 * slot);
-          }
+          mbar_wait(bar_bempty + 8 * slot, ph ^ 1u);
+          mbar_arrive_expect_tx(bar_bfull + 8 * slot, p.b_slot_bytes);
+          bulk_g2s(b_smem + slot * p.b_slot_bytes, wsrc + (size_t)j * p.b_slot_bytes, p.b_slot_bytes, bar_bfull + 8 * slot);
           ring_next(slot, ph, (uint32_t)p.b_slots);
         }
       }
     }
-    __syncwarp();
-  } else {
-    // ======================================================= epilogue (warps 0..15)
-    const int q = warp & 3;   // TMEM lane quarter
-    const int g = warp >> 2;  // group
-    float* ss = reinterpret_cast<float*>(smem + p.off_ss);
-    for (int i = threadIdx.x; i < p.n_cta; i += 32 * kSEpiWarps) ss[i] = p.shift[split * p.n_cta + i];
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * kSEpiWarps) : "memory");
-    asm volatile("griddepcontrol.wait;" ::: "memory");  // our stores may overwrite what the previous kernel still reads
-    if (g < mt * nsets) {
-      const int set = g / mt, t = g - set * mt;
-      const int r = q * 32 + lane;  // accumulator row == TMEM lane == tile cell
-      const int py = r >> 3, px = r & 7;
-      const int n0 = split * p.n_cta;
-      const int nchunks = p.n_cta >> 4;
-      const float slope = p.act ? 0.2f : 1.f;  // max(a, slope * a): LeakyReLU(0.2) or identity
-      const uint32_t taddr = tmem_base + (uint32_t)(set * mt + t) * p.acc_stride + ((uint32_t)(q * 32) << 16);
-      for (int k = set; k < my_passes; k += nsets) {
-        const int pass = pass0 + k * pass_stride;
-        const TileCoord tc = tile_coord(p, pass * mt + t);
-        const int gy = tc.ty * kTileH + py, gx = tc.tx * kTileW + px;
-        const bool valid = (tc.b < p.B) && (gy < p.H) && (gx < p.W);
-        mbar_wait(bar_tfull + 8 * set, (uint32_t)((k / nsets) & 1), 17);
-        tc_fence_after();
-        const size_t opix = valid ? (((size_t)tc.b * p.H + gy) * p.W + gx) * (size_t)p.out_pitch + (size_t)n0 : 0;
-        T* orow = reinterpret_cast<T*>(p.out) + opix;
-        const T* rrow = reinterpret_cast<const T*>(p.res) + opix;  // EXT only
-        for (int c = 0; c < nchunks; c += 2) {
-          uint32_t v0[16], v1[16];
-          const bool two = (c + 1 < nchunks);
-          tmem_ld16(taddr + c * 16, v0);
-          if (two) tmem_ld16(taddr + (c + 1) * 16, v1);
-          tmem_ld_wait();
-          if (c + 2 >= nchunks) {  // the accumulator has been read completely
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_tempty + 8 * set);
-          }
-          auto finish = [&](int cc, const uint32_t(&vv)[16]) {
-            const float4* sp = reinterpret_cast<const float4*>(ss + cc * 16);
-            const float4 s0 = sp[0], s1 = sp[1], s2 = sp[2], s3 = sp[3];
-            const float shf[16] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w,
-                                   s2.x, s2.y, s2.z, s2.w, s3.x, s3.y, s3.z, s3.w};
-            uint32_t o[8];
-            if constexpr (EXT) {
-              uint4 r0 = make_uint4(0u, 0u, 0u, 0u), r1 = r0;
-              if (p.res != nullptr && valid) {
-                r0 = *reinterpret_cast<const uint4*>(rrow + cc * 16);
-                r1 = *reinterpret_cast<const uint4*>(rrow + cc * 16 + 8);
-              }
-              const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-              const float ps = p.slope;
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float a0 = __uint_as_float(vv[2 * j]) + shf[2 * j];
-                float a1 = __uint_as_float(vv[2 * j + 1]) + shf[2 * j + 1];
-                a0 = a0 > 0.f ? a0 : ps * a0;
-                a1 = a1 > 0.f ? a1 : ps * a1;
-                const float2 rf = Pack2<T>::unpack(rw[j]);
-                o[j] = Pack2<T>::pack(a0 + rf.x, a1 + rf.y);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float a0 = __uint_as_float(vv[2 * j]) + shf[2 * j];
-                const float a1 = __uint_as_float(vv[2 * j + 1]) + shf[2 * j + 1];
-                o[j] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
-              }
-            }
-            if (valid) stg256(orow + cc * 16, o);  // 32 contiguous, 32-byte aligned bytes (pitch and n0 multiples of 16)
-          };
-          finish(c, v0);
-          if (two) finish(c + 1, v1);
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  if constexpr (CL == 2)
-    cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
-  else
-    __syncthreads();
-  if (warp == kSMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
+  // ========================================================= MMA + epilogue warpgroups (warpgroup t = tile t of a pass)
+  const int t = warp >> 2;
+  const int wq = warp & 3;
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // our stores may overwrite what the previous kernel still reads
+  const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);   // LBO(=1) | start address, 16-byte units
+  const uint32_t b_lo0 = (1u << 16) | (b_smem >> 4);
+  const uint32_t b_hi = (1024u >> 4) | kDescSw128;     // SBO = 8 rows x 128 B, SWIZZLE_128B
+  const uint32_t a_hi = p.a_hi;                        // SBO = halo_w x 128 B, SWIZZLE_128B
+  const uint32_t half_off = 8u * (a_hi & 0x3fffu);      // rows 64..127 of the tile: 8 tile rows further down
+  const uint32_t a_slot_u = p.a_slot_bytes >> 4, a_win_u = p.a_win_bytes >> 4, b_slot_u = p.b_slot_bytes >> 4;
+  const int n0 = split * p.n_cta;
+  const float slope = p.act ? 0.2f : 1.f;  // max(a, slope * a): LeakyReLU(0.2) or identity
+  const int px = lane >> 2, c2 = 2 * (lane & 3);
+  uint32_t aslot = 0, aph = 0, bslot = 0, bph = 0;
+  float acc[2][N / 2];
+  for (int k = 0; k < my_passes; ++k) {
+    // MMAs of one (k-block, tap) form one wgmma group; the slot of the previous group is released once it completes
+    uint32_t prev_b = 0, prev_a = 0;
+    bool prev_last_tap = false, have_prev = false;
+    for (int kb = 0; kb < p.nkb; ++kb) {
+      mbar_wait(bar_afull + 8 * aslot, aph);
+      for (int tap = 0; tap < p.ntaps; ++tap) {
+        mbar_wait(bar_bfull + 8 * bslot, bph);
+        wgmma_fence();
+        const uint32_t a_lo = a_lo0 + aslot * a_slot_u + (uint32_t)t * a_win_u + p.tap_off[tap];
+        const uint32_t b_lo = b_lo0 + bslot * b_slot_u;
+        const uint32_t first_mma = (kb | tap) ? 1u : 0u;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint64_t a64 = ((uint64_t)a_hi << 32) | (uint64_t)(a_lo + (uint32_t)h * half_off);
+          uint64_t b64 = ((uint64_t)b_hi << 32) | (uint64_t)b_lo;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {  // 64 channels = four K=16 steps, +32 B each
+            wgmma_ss<N, T>(acc[h], a64, b64, i ? 1u : first_mma);
+            a64 += 2;
+            b64 += 2;
+          }
+        }
+        wgmma_commit();
+        if (have_prev) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(bar_bempty + 8 * prev_b);
+            if (prev_last_tap) mbar_arrive(bar_aempty + 8 * prev_a);
+          }
+        }
+        have_prev = true;
+        prev_b = bslot;
+        prev_a = aslot;
+        prev_last_tap = (tap == p.ntaps - 1);
+        ring_next(bslot, bph, (uint32_t)p.b_slots);
+      }
+      ring_next(aslot, aph, (uint32_t)p.a_slots);
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(bar_bempty + 8 * prev_b);
+      mbar_arrive(bar_aempty + 8 * prev_a);
+    }
+    acc_fence(acc[0]);
+    acc_fence(acc[1]);
+
+    // ---- epilogue: d[h][4 j + 2 e + c] = tile row 8 h + 2 wq + e, column 8 j + c2 + c
+    const TileCoord tc = tile_coord(p, (pass0 + k * pass_stride) * mt + t);
+    if (tc.b >= p.B) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int gy = tc.ty * kTileH + 8 * h + 2 * wq + e, gx = tc.tx * kTileW + px;
+        if (gy >= p.H || gx >= p.W) continue;
+        const size_t opix = (((size_t)tc.b * p.H + gy) * p.W + gx) * (size_t)p.out_pitch + (size_t)n0;
+        T* orow = reinterpret_cast<T*>(p.out) + opix;
+        const T* rrow = reinterpret_cast<const T*>(p.res) + opix;  // EXT only
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          const int n = 8 * j + c2;
+          const float2 sh = *reinterpret_cast<const float2*>(p.shift + n0 + n);
+          float a0 = acc[h][4 * j + 2 * e] + sh.x, a1 = acc[h][4 * j + 2 * e + 1] + sh.y;
+          uint32_t o;
+          if constexpr (EXT) {
+            a0 = a0 > 0.f ? a0 : p.slope * a0;
+            a1 = a1 > 0.f ? a1 : p.slope * a1;
+            if (p.res != nullptr) {
+              const float2 rf = Pack2<T>::unpack(*reinterpret_cast<const uint32_t*>(rrow + n));
+              a0 += rf.x;
+              a1 += rf.y;
+            }
+            o = Pack2<T>::pack(a0, a1);
+          } else {
+            o = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+          }
+          *reinterpret_cast<uint32_t*>(orow + n) = o;
+        }
+      }
   }
 }
 
@@ -449,36 +377,18 @@ bool streamconv_plan(const StreamConvLayer& L, StreamConvParams* pp) {
   p.nkb = (L.c0 + L.c1) / 64;
   p.n_total = L.n_total;
   p.act = L.act;
-  // output channels per CTA: the whole layer up to 128, else 128-wide splits (n_total = 256, 512).  SC_NCTA=256 selects
-  // 256-wide CTAs (one accumulator set, no epilogue overlap) for A/B runs.
-  static const int want_ncta = [] {
-    const char* e = std::getenv("VFI_SC_NCTA");
-    return (e && std::atoi(e) == 256) ? 256 : 128;
-  }();
-  int n_cta = L.n_total;
-  if (n_cta > want_ncta) n_cta = want_ncta;
+  // output channels per CTA (the wgmma N): the whole layer up to 128, else 128-wide splits (n_total = 256, 512)
+  int n_cta = L.n_total < 128 ? L.n_total : 128;
   while (L.n_total % n_cta) n_cta -= 16;
   p.n_cta = n_cta;
   p.nsplit = L.n_total / n_cta;
-  static const int want_mt = [] {
-    const char* e = std::getenv("VFI_SC_MT");
-    return (e && e[0] == '1') ? 1 : 2;
-  }();
-  p.mt = want_mt;
-  uint32_t stride = 32;
-  while (stride < (uint32_t)n_cta) stride <<= 1;
-  p.acc_stride = stride;
-  p.nsets = (p.mt * 2 * (int)stride <= 512) ? 2 : 1;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(p.mt * p.nsets) * stride) cols <<= 1;
-  p.tmem_cols = cols;
+  p.mt = kSMmaGroups;  // one tile per MMA warpgroup
   p.b_slot_bytes = (uint32_t)n_cta * 128u;
   p.w_split_bytes = (size_t)p.nkb * p.ntaps * p.b_slot_bytes;
   p.a_tx_bytes = (uint32_t)p.halo_w * (uint32_t)p.halo_h * 128u;
   p.a_win_bytes = sc_align_up(p.a_tx_bytes, 1024);
   p.a_slot_bytes = (uint32_t)p.mt * p.a_win_bytes;
-  p.off_ss = kSCtrlBytes;
-  p.off_b = sc_align_up(p.off_ss + (uint32_t)n_cta * 4u, 1024);
+  p.off_b = sc_align_up(kSCtrlBytes, 1024);
   // shared memory: at least 2 window slots and 3 weight slots; then a third window slot if 4 weight slots still fit;
   // the rest goes to weight slots (a window slot lasts ntaps x mt x 4 MMAs, a weight slot mt x 4)
   int a_slots = 2;
@@ -493,7 +403,7 @@ bool streamconv_plan(const StreamConvLayer& L, StreamConvParams* pp) {
   p.b_slots = b_slots;
   p.off_a = p.off_b + (uint32_t)b_slots * p.b_slot_bytes;  // multiples of 2048: 1024-aligned
   p.smem_bytes = p.off_a + (uint32_t)a_slots * p.a_slot_bytes;
-  p.a_hi = (((uint32_t)p.halo_w * 128u) >> 4) | (1u << 14) | (2u << 29);
+  p.a_hi = (((uint32_t)p.halo_w * 128u) >> 4) | kDescSw128;
   for (int tap = 0; tap < p.ntaps; ++tap)
     p.tap_off[tap] = ((uint32_t)((tap / L.ksize) * p.halo_w + (tap % L.ksize)) * 128u) >> 4;
   return true;
@@ -575,8 +485,6 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
   p.tiles_x = (W + kTileW - 1) / kTileW;
   p.ntiles = B * p.tiles_y * p.tiles_x;
   p.npasses = (p.ntiles + p.mt - 1) / p.mt;
-  const uint32_t fmt = (op_type == OP_BF16) ? 1u : 0u;
-  p.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(p.n_cta >> 3) << 17) | ((128u >> 4) << 24);
 
   if (use_ref) {
     const size_t total = (size_t)B * H * W * L.n_total;
@@ -599,17 +507,11 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
   } else {
     p.tm[1] = p.tm[0];
   }
-  static const int cluster = [] {  // VFI_SC_CLUSTER=2: two-CTA clusters sharing the weight stream by multicast (never run yet)
-    const char* e = std::getenv("VFI_SC_CLUSTER");
-    return (e && e[0] == '2') ? 2 : 1;
-  }();
-  const int cl = (cluster == 2 && p.npasses >= 2) ? 2 : 1;
-  const int units = cl == 2 ? (p.npasses + 1) / 2 : p.npasses;  // passes, or pass pairs (one per cluster)
-  int cps = num_sms / cl / p.nsplit;                             // CTAs (clusters) per output-channel split
+  int cps = num_sms / p.nsplit;  // persistent CTAs per output-channel split
   if (cps < 1) cps = 1;
-  if (cps > units) cps = units;
+  if (cps > p.npasses) cps = p.npasses;
   p.ctas_per_split = cps;
-  const int grid = cps * p.nsplit * cl;
+  const int grid = cps * p.nsplit;
   static const bool pdl = [] {
     const char* e = std::getenv("VFI_PDL");
     return !(e && e[0] == '0');
@@ -622,33 +524,35 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
     cfg.blockDim = dim3((unsigned)kSThreads);
     cfg.dynamicSmemBytes = p.smem_bytes;
     cfg.stream = st;
-    cudaLaunchAttribute attr[2];
+    cudaLaunchAttribute attr[1];
     int na = 0;
     if (pdl) {
       attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       attr[na].val.programmaticStreamSerializationAllowed = 1;
       ++na;
     }
-    if (cl == 2) {
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = 2;
-      attr[na].val.clusterDim.y = 1;
-      attr[na].val.clusterDim.z = 1;
-      ++na;
-    }
     cfg.attrs = attr;
     cfg.numAttrs = na;
     return cudaLaunchKernelEx(&cfg, kern, p);
   };
-  cudaError_t err;
-  if (cl == 2 && L.ext)
-    err = (op_type == OP_BF16) ? go(streamconv_kernel<__nv_bfloat16, true, 2>) : go(streamconv_kernel<__half, true, 2>);
-  else if (cl == 2)
-    err = (op_type == OP_BF16) ? go(streamconv_kernel<__nv_bfloat16, false, 2>) : go(streamconv_kernel<__half, false, 2>);
-  else if (L.ext)
-    err = (op_type == OP_BF16) ? go(streamconv_kernel<__nv_bfloat16, true, 1>) : go(streamconv_kernel<__half, true, 1>);
-  else
-    err = (op_type == OP_BF16) ? go(streamconv_kernel<__nv_bfloat16, false, 1>) : go(streamconv_kernel<__half, false, 1>);
+  auto pick_n = [&](auto tag, auto ext) -> cudaError_t {
+    using T = decltype(tag);
+    constexpr bool X = decltype(ext)::value;
+    switch (p.n_cta) {  // streamconv_plan: a multiple of 16 up to 128
+      case 16: return go(streamconv_kernel<T, X, 16>);
+      case 32: return go(streamconv_kernel<T, X, 32>);
+      case 48: return go(streamconv_kernel<T, X, 48>);
+      case 64: return go(streamconv_kernel<T, X, 64>);
+      case 80: return go(streamconv_kernel<T, X, 80>);
+      case 96: return go(streamconv_kernel<T, X, 96>);
+      case 112: return go(streamconv_kernel<T, X, 112>);
+      default: return go(streamconv_kernel<T, X, 128>);
+    }
+  };
+  auto pick = [&](auto tag) -> cudaError_t {
+    return L.ext ? pick_n(tag, std::true_type{}) : pick_n(tag, std::false_type{});
+  };
+  const cudaError_t err = (op_type == OP_BF16) ? pick(__nv_bfloat16{}) : pick(__half{});
   if (err != cudaSuccess) return err;
   return cudaGetLastError();
 #endif  // VFI_HOST_EMU

@@ -1,34 +1,29 @@
-// tapconv: tap-list implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05 / TMEM / TMA), sm_100a only.
+// tapconv: tap-list implicit-GEMM convolution on the Hopper tensor cores (wgmma / TMA / mbarrier), sm_90a only.
 //
 // Replaces, for the RIFE IFBlock (reference rife_arch.py:237-276), the cuDNN/ATen kernels behind
 //   conv0.0 / conv0.1  Conv2d(3x3, stride 2)+LeakyReLU        rife_arch.py:96-107, :181-184
 //   convblock          8 x ResConv  lrelu(conv3x3(x)*beta + x) rife_arch.py:20-28, :201-210
 //   lastconv           ConvTranspose2d(c,24,4,2,1)+PixelShuffle rife_arch.py:215-218
 //
-// One CTA tile = 16 x 8 grid cells = the M=128 rows of one tcgen05.mma.  The input window of the tile
-// (tile + halo, all input channels) is dropped ONCE into shared memory by TMA as rows of 64 channels
+// One CTA tile = 16 x 8 grid cells = 128 GEMM rows, two m64 wgmma row blocks (tile rows 0-7 and 8-15).  The input
+// window of the tile (tile + halo, all input channels) is dropped ONCE into shared memory by TMA as rows of 64 channels
 //      A[k-block][window pixel][64 ch = 128 B, SWIZZLE_128B]      (a 32-channel SWIZZLE_64B tail when cin % 64 = 32)
-// i.e. the canonical K-major swizzled UMMA operand with "rows = pixels".  TMA zero-fills everything outside the
+// i.e. the canonical K-major swizzled wgmma operand with "rows = pixels".  TMA zero-fills everything outside the
 // image, which implements both the convolution padding and partial border tiles.  Every filter tap is then just a
 // different descriptor START ADDRESS into the same window (whole-row shift (dy*halo_w + dx) * 128 B, with the
 // 8-row-group stride SBO = halo_w * 128 B), a K=16 step a 32-byte shift inside the row: the tensor core applies the
-// 128B XOR swizzle on the absolute shared-memory address, exactly where TMA put the data (verified on B200, r01:
-// unaligned start addresses and SBO = 1280 B work with base_offset = 0).  So the 3x3 window is read from L2 once
-// (x1.41 halo), not 9x as with im2col.  Weights of the CTA's output-channel slice are resident in shared memory for
-// the whole launch (one bulk copy, already in the swizzled operand layout), accumulators live in TMEM (double
-// buffered), the epilogue reads the ResConv residual back from the staged window instead of from global memory.
+// XOR swizzle on the absolute shared-memory address, exactly where TMA put the data.  So the 3x3 window is read from L2
+// once (x1.41 halo), not 9x as with im2col.  Weights of the CTA's output-channel slice are resident in shared memory
+// for the whole launch (one bulk copy, already in the swizzled operand layout).
 //
-// Warp roles (576 threads, 1 CTA/SM, persistent over tiles):
-//   warps 0..15 : epilogue - four sets of four warps (TMEM lane quarters 0..3).  Sets {0,1} take the even tiles of
-//                 the CTA (TMEM accumulator 0), sets {2,3} the odd ones (accumulator 1); inside a pair each set takes
-//                 half of the accumulator columns: tcgen05.ld -> release TMEM -> +shift (+residual) -> LeakyReLU
-//                 -> 16-bit -> global stores (lastconv: the fp32 4x4 flow/mask sub-pixel patch).
-//                 (ncu r01_v11: with 8 epilogue warps each warp needed ~480 dependent instructions per tile at ~9
-//                 cycles each = the whole tile time, while the tensor pipe was 14 % busy; tools/mma_rate.cu: the
-//                 hardware floor for an N=64 MMA of this form is 48 cycles.)
-//   warp 16     : TMEM alloc/dealloc; one elected lane issues tcgen05.mma + tcgen05.commit
-//   warp 17     : one elected lane: weight bulk copy, then one 4-D TMA tensor copy per k-block and tile
+// Warp roles (288 threads, 1 CTA/SM, persistent over tiles):
+//   warpgroups 0, 1 : MMA + epilogue.  Warpgroup w takes the CTA's tiles w, w + 2, ... and keeps the whole tile's
+//                     accumulators (2 x 64 rows x n_cta columns, fp32) in registers, so one warpgroup's epilogue
+//                     (+shift (+residual) -> LeakyReLU -> 16-bit -> global stores; lastconv: the fp32 4x4 flow/mask
+//                     sub-pixel patch) overlaps the other's MMAs.
+//   warp 8          : one elected lane: weight bulk copy, then one 4-D TMA tensor copy per k-block and tile
 #include <cstdlib>
+#include <type_traits>
 
 #include "ptx.cuh"
 #include "vfi_internal.h"
@@ -37,21 +32,14 @@ namespace vfi {
 
 namespace {
 
-constexpr int kMaxStages = 6;   // window stages (<= 4 used) or ring slots
-constexpr int kAccBufs = 4;     // TMEM accumulator buffers == epilogue groups
-constexpr int kDefaultStoreMode = 2;  // see VFI_STORE in tapconv_plan
-constexpr int kDefaultMaxStages = 4;  // window stages of the non-ring layers (VFI_STAGES_MAX = 1..6 for A/B runs)
+constexpr int kMaxStages = 6;   // window stages or ring slots
 struct Ctrl {
   uint64_t w_full;
-  uint64_t w_peer;  // pair mode, leader CTA only: the follower's weights have landed (remote arrive)
-  uint64_t a_full[kMaxStages];
+  uint64_t a_full[kMaxStages][2];  // [stage][consuming warpgroup]
   uint64_t a_empty[kMaxStages];
-  uint64_t t_full[kAccBufs];
-  uint64_t t_empty[kAccBufs];
-  uint32_t tmem_base;
 };
 constexpr uint32_t kCtrlBytes = 256;
-constexpr int kEpiWarps = 16, kMmaWarp = 16, kMmaWarp2 = 17, kTmaWarp = 18, kThreads = 32 * 19;
+constexpr int kMmaGroups = 2, kTmaWarp = 8, kThreads = 128 * kMmaGroups + 32;
 static_assert(sizeof(Ctrl) <= kCtrlBytes, "control block");
 
 __device__ __forceinline__ size_t out_pixel_offset(const TapConvParams& p, int b, int gy, int gx) {
@@ -66,7 +54,7 @@ __device__ __forceinline__ size_t out_pixel_offset(const TapConvParams& p, int b
   return (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.n_total;
 }
 
-#ifndef VFI_HOST_EMU  // (tests/host_emu runs the RIFE schedule on the CPU with the checker kernel; no tcgen05 there)
+#ifndef VFI_HOST_EMU  // (tests/host_emu runs the RIFE schedule on the CPU with the checker kernel; no wgmma there)
 // Walks the tiles of one CTA (t = first, first + cps, ...) keeping (image, tile row, tile column) incrementally
 // instead of two integer divisions per tile and role.
 struct TileIter {
@@ -99,563 +87,225 @@ struct TileIter {
   }
 };
 
-// One tile's MMAs as NR "runs" of L consecutive K=16 steps (same tap, same k-block: both descriptors advance by
-// 32 bytes per step).  NR and L are compile-time constants, so every p.mma[r] is a fixed constant-bank address and the
-// steps inside a run are immediate adds: ~4.7 SASS instructions per MMA for L = 4 (r01_v11: a table entry per step
-// cost 8-15 - LDC/IMAD/R2UR chains - and the issuing warp, not the tensor pipe, set the tile time).
-template <int NR, int L, bool PAIR>
-__device__ __forceinline__ void issue_runs(const TapConvParams& p, uint32_t d_tmem, uint32_t a_lo0, uint32_t b_lo0,
-                                           uint32_t b_hi, uint32_t idesc, uint32_t accumulate_first = 0u) {
-#pragma unroll
-  for (int r = 0; r < NR; ++r) {
+// One window's MMAs for both 64-row halves of the tile: p.nruns runs of p.run_len consecutive K=16 steps (same tap,
+// same k-block: both descriptors advance by 32 bytes per step).  a_base / b_base: start-address words (16-byte units,
+// LBO = 1) of the window and of the weights of this k-block.
+template <int N, typename T>
+__device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc)[2][N / 2], uint32_t a_base,
+                                             uint32_t b_base, uint32_t accumulate_first) {
+#pragma unroll 1
+  for (int r = 0; r < p.nruns; ++r) {
     const uint4 d = p.mma[r];
-    // whole 64-bit descriptors advanced in place (+32 B per K=16 step): each stays in one uniform register pair, no
-    // per-MMA re-packing of {lo, hi} (r01: that cost UMOVs and uniform-register spills, ~83 cycles of issue per MMA)
-    uint64_t a64 = ((uint64_t)d.y << 32) | (uint64_t)(a_lo0 + d.x);
-    uint64_t b64 = ((uint64_t)b_hi << 32) | (uint64_t)(b_lo0 + d.z);
+    const uint32_t half_off = 8u * (d.y & 0x3fffu);  // 8 tile rows further down the window = 8 SBO strides
 #pragma unroll
-    for (int i = 0; i < L; ++i) {
-      if (PAIR)
-        umma_f16_pair(d_tmem, a64, b64, idesc, (r | i) ? 1u : accumulate_first);
-      else
-        umma_f16(d_tmem, a64, b64, idesc, (r | i) ? 1u : accumulate_first);
-      a64 += 2;
-      b64 += 2;
-    }
-  }
-}
-
-struct MmaLoopArgs {
-  uint32_t bar_tfull, bar_tempty, bar_afull, bar_aempty;  // shared-memory addresses of the barrier arrays
-  uint32_t tmem_base, a_base, b_lo0, b_hi;
-  int ntiles;        // tiles of this CTA
-  uint32_t S;        // window stages / ring slots
-  bool commit_stage; // the MMA commit releases the window stage (false: the epilogue does, after reading the residual)
-};
-
-// Diagnostic build only (-DVFI_ABLATE, tools/ablate.py): p.ablate switches parts of the pipeline off so that the tile time
-// of what remains can be measured.  1: no epilogue global stores / residual loads, 2: epilogue = tcgen05.ld + barrier
-// hand-shake only, 4: no tcgen05.ld either, 8: producer signals "full" without issuing TMA, 16: no tcgen05.mma,
-// 32 / 64: the MMA warp does not wait for the accumulator / the window, 256: no tcgen05.fence in its loop, 512: no
-// tcgen05.commit, 1024: only the MMA warps run (results are garbage, timing only).
-#ifdef VFI_ABLATE
-#define ABLATE(bit) ((p.ablate & (bit)) != 0)
-#else
-#define ABLATE(bit) false
-#endif
-
-// An issuing thread's whole life.  With an even number of window stages TWO threads (one lane of warp 16, one of
-// warp 17) share the work: thread `which` takes the CTA's tiles which, which + 2, ... and with them TMEM accumulator
-// `which` and the window stages of its parity - every barrier keeps exactly one waiter that sees each of its phases
-// in turn (an mbarrier parity wait cannot tell phase n from n + 2).  Ring layers and odd stage counts use one thread.  While one of them sits in its
-// commit / fence / barrier waits (~600 cycles per tile, r01 ablation, with a tensor-pipe queue only a few MMAs deep)
-// the other one keeps the pipe fed.  Per tile: wait for the free accumulator and the full window (ring layers: k-block
-// slot by slot), issue the MMAs, commit.
-__device__ __forceinline__ void advance_stage(uint32_t& stage, uint32_t& ph, uint32_t n, uint32_t S) {
-  stage += n;
-  while (stage >= S) {
-    stage -= S;
-    ph ^= 1u;
-  }
-}
-
-template <bool PAIR>
-__device__ __forceinline__ void commit_to(uint32_t bar) {
-  if (PAIR)
-    umma_commit_pair(bar);  // the same barrier offset in both CTAs of the pair
-  else
-    umma_commit(bar);
-}
-
-template <int NR, int L, bool RING, bool PAIR>
-__device__ __forceinline__ void mma_tile_loop(const TapConvParams& p, const MmaLoopArgs& g, uint32_t which,
-                                              uint32_t nissuers) {
-  const uint32_t idesc = p.idesc;
-  const uint32_t stage_units = p.stage_bytes >> 4;
-  uint32_t stage = 0, aph = 0;                            // window stage / ring slot and its "full" parity
-  const uint32_t per_tile = RING ? (uint32_t)p.nkb : 1u;  // stages / slots one tile consumes
-  advance_stage(stage, aph, which * per_tile, g.S);
-  const uint32_t b_kb = (9u * (uint32_t)p.n_cta * 128u) >> 4;  // ring: weight bytes of one k-block, 16-byte units
-  for (uint32_t k = which; k < (uint32_t)g.ntiles; k += nissuers) {
-    const uint32_t acc = k % kAccBufs;  // accumulator buffer; its "empty" barrier is waited with parity (uses & 1) ^ 1
-    const uint32_t d_tmem = g.tmem_base + acc * p.acc_stride;
-    if (!ABLATE(32)) {
-      if (PAIR)  // both CTAs' epilogue groups have drained this accumulator (the follower's arrive remotely)
-        mbar_wait_cluster(g.bar_tempty + 8 * acc, ((k / kAccBufs) & 1u) ^ 1u, 2);
-      else
-        mbar_wait(g.bar_tempty + 8 * acc, ((k / kAccBufs) & 1u) ^ 1u, 2);
-    }
-    if (RING) {
-      for (int kb = 0; kb < p.nkb; ++kb) {
-        mbar_wait(g.bar_afull + 8 * stage, aph, 3);
-        tc_fence_after();
-        issue_runs<NR, L, PAIR>(p, d_tmem, g.a_base + stage * stage_units, g.b_lo0 + (uint32_t)kb * b_kb, g.b_hi, idesc,
-                                kb > 0 ? 1u : 0u);
-        commit_to<PAIR>(g.bar_aempty + 8 * stage);
-        advance_stage(stage, aph, 1u, g.S);
+    for (int h = 0; h < 2; ++h) {
+      uint64_t a64 = ((uint64_t)d.y << 32) | (uint64_t)(a_base + d.x + (uint32_t)h * half_off);
+      uint64_t b64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b_base + d.z);
+#pragma unroll 1
+      for (int i = 0; i < p.run_len; ++i) {
+        wgmma_ss<N, T>(acc[h], a64, b64, (r | i) ? 1u : accumulate_first);
+        a64 += 2;
+        b64 += 2;
       }
-      commit_to<PAIR>(g.bar_tfull + 8 * acc);
-      if (nissuers > 1) advance_stage(stage, aph, per_tile, g.S);  // the other thread's tile
-    } else {
-      if (!ABLATE(64)) mbar_wait(g.bar_afull + 8 * stage, aph, 3);
-      if (!ABLATE(256)) tc_fence_after();
-      if (!ABLATE(16)) issue_runs<NR, L, PAIR>(p, d_tmem, g.a_base + stage * stage_units, g.b_lo0, g.b_hi, idesc);
-      if (!ABLATE(512)) {
-        if (g.commit_stage) commit_to<PAIR>(g.bar_aempty + 8 * stage);  // window free once the MMAs have read it
-        commit_to<PAIR>(g.bar_tfull + 8 * acc);                          // accumulator ready for the epilogue
-      }
-      advance_stage(stage, aph, nissuers, g.S);
     }
   }
 }
 
-template <typename T, bool RING, bool LAST, bool PAIR>
+template <typename T, bool RING, bool LAST, int N>
 __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_constant__ TapConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   // Programmatic dependent launch (launch_tapconv sets the attribute): the next kernel in the stream may start its
   // CTAs as soon as every CTA of this grid has passed this point, i.e. while our last tiles are still running - they do
-  // their prologue (barrier init, TMEM allocation, weight copy) on the SMs our first finishers free and then block in
+  // their prologue (barrier init, weight copy) on the SMs our first finishers free and then block in
   // griddepcontrol.wait until this grid has completed and flushed.  Both instructions are no-ops without the attribute.
   asm volatile("griddepcontrol.launch_dependents;");
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // Work assignment.  Single CTAs: CTA (split, first) takes the output-channel slice `split` of tiles first, first + cps,
-  // ...  CTA PAIRS (PAIR, a cluster of two CTAs = the two SMs of a TPC): pair (split, pi) takes the TILE PAIRS pi,
-  // pi + pps, ...; rank r of the pair owns tile 2 * j + r of tile pair j, its own window of it and ITS HALF (n_cta rows,
-  // packed slice 2 * split + r) of the B operand; one tcgen05.mma.cta_group::2 (M = 256, N = n_epi = 2 * n_cta) issued
-  // by rank 0 multiplies both windows with both halves and leaves each CTA's tile, all n_epi columns, in that CTA's own
-  // TMEM.  Per MMA a CTA's shared memory is read for 128 x 32 B of A and only n_cta x 32 B of B: for c = 64 that is 40
-  // instead of 48 wavefronts against 32 cycles of math (the r01 limiter), for c >= 96 the MMA is math bound; the
-  // per-tile issue / fence / commit cost of the issuing thread is paid once per TWO tiles; and the wide layers need
-  // half as many output-channel splits.  If the tile count is odd the last tile of rank 1 is a dummy: its window
-  // coordinates are outside the tensor (TMA fills zeros) and its epilogue stores nothing.
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int unit = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;  // pair index / CTA index in the grid
-  const int nsplit_u = PAIR ? (p.nsplit >> 1) : p.nsplit;            // output-channel splits of the grid
-  const int split = unit % nsplit_u;
-  const int ufirst = unit / nsplit_u;
-  if (!PAIR && ufirst >= p.ctas_per_split) return;  // whole CTA leaves together (never taken in pair mode)
-  const int first = PAIR ? 2 * ufirst + (int)rank : ufirst;                  // this CTA's first tile ...
-  const int tstep = PAIR ? 2 * p.ctas_per_split : p.ctas_per_split;           // ... and its stride
-  const int nunits = PAIR ? (p.ntiles + 1) >> 1 : p.ntiles;                   // tile pairs / tiles of the layer
-  const int my_tiles = (nunits - ufirst + p.ctas_per_split - 1) / p.ctas_per_split;  // same for both ranks of a pair
-  const int wslice = PAIR ? 2 * split + (int)rank : split;                    // packed weight slice of this CTA
-  const int n0 = split * p.n_epi;                                             // first output channel of the epilogue
+  // CTA (split, first) takes the output-channel slice `split` of tiles first, first + cps, ...
+  const int split = (int)blockIdx.x % p.nsplit;
+  const int first = (int)blockIdx.x / p.nsplit;
+  if (first >= p.ctas_per_split) return;  // whole CTA leaves together
+  const int tstep = p.ctas_per_split;
+  const int my_tiles = (p.ntiles - first + tstep - 1) / tstep;
+  const int n0 = split * p.n_cta;  // first output channel of this CTA
   const int S = p.stages;
   const bool residual = !LAST && (p.epi_mode == EPI_RESCONV);
-  const bool res_smem = residual && !RING;  // ring layers read the residual from global memory (L2 hit)
 
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_w = smem_base + offsetof(Ctrl, w_full);
-  const uint32_t bar_wpeer = smem_base + offsetof(Ctrl, w_peer);
   const uint32_t bar_afull = smem_base + offsetof(Ctrl, a_full);
   const uint32_t bar_aempty = smem_base + offsetof(Ctrl, a_empty);
-  const uint32_t bar_tfull = smem_base + offsetof(Ctrl, t_full);
-  const uint32_t bar_tempty = smem_base + offsetof(Ctrl, t_empty);
   const uint32_t a_smem = smem_base + p.off_a;
   const uint32_t w_smem = smem_base + p.off_w;
   const bool has_tail = (p.cin & 63) != 0;  // last k-block is 32 channels wide
 
   if (threadIdx.x == 0) {
     mbar_init(bar_w, 1);
-    mbar_init(bar_wpeer, 1);
     for (int s = 0; s < S; ++s) {
-      mbar_init(bar_afull + 8 * s, 1);                  // producer's arrive.expect_tx (+ TMA transaction bytes)
-      mbar_init(bar_aempty + 8 * s, (residual && !RING) ? 4 : 1);  // the tile's 4 epilogue warps, or the MMA commit
-    }
-    for (int a = 0; a < kAccBufs; ++a) {
-      mbar_init(bar_tfull + 8 * a, 1);
-      mbar_init(bar_tempty + 8 * a, PAIR ? 8 : 4);  // the four warps of the accumulator's epilogue group (of both CTAs)
+      mbar_init(bar_afull + 16 * s, 1);      // producer's arrive.expect_tx (+ TMA transaction bytes), per warpgroup
+      mbar_init(bar_afull + 16 * s + 8, 1);
+      mbar_init(bar_aempty + 8 * s, 4);      // the four warps of the consuming warpgroup
     }
     mbar_fence_init();
   }
-  if (warp == kMmaWarp) {
-    if (PAIR)
-      tmem_alloc_pair(smem_base + offsetof(Ctrl, tmem_base), p.tmem_cols);
-    else
-      tmem_alloc(smem_base + offsetof(Ctrl, tmem_base), p.tmem_cols);
-  }
-  tc_fence_before();
-  if (PAIR)
-    cluster_sync_all();  // the peer's barriers are initialised before anything of ours signals them
-  else
-    __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
+  __syncthreads();
 
-  if (warp == kMmaWarp || warp == kMmaWarp2) {
-    // ======================================================= MMA issuers
-    // ONE elected lane per issuing warp runs its tile loop (the other lanes go straight to the final barrier).  Per tile it does
-    // two mbarrier waits, the fence, the unrolled MMAs and the commits - nothing else: stage / phase / accumulator
-    // state is carried incrementally and the issue shape is dispatched once, outside the loop (r01 ablation: with a
-    // division, a switch and warp re-convergence per tile the loop cost 660 cycles per tile on top of the MMAs, none
-    // of it overlapped with the tensor pipe, whose queue is only a few MMAs deep).
-    if (PAIR && rank != 0) {
-      // follower CTA: its second issuing warp only tells the leader when this CTA's half of the weights has landed
-      if (warp == kMmaWarp2 && elect_one_sync() && !ABLATE(1024)) {
-        mbar_wait(bar_w, 0, 1);
-        mbar_arrive_remote(mapa_u32(bar_wpeer, 0));
-      }
-    } else if (elect_one_sync()) {
-      if (!ABLATE(1024)) {
-        mbar_wait(bar_w, 0, 1);
-        if (PAIR && warp == kMmaWarp) mbar_wait_cluster(bar_wpeer, 0, 7);
-      }
-      const uint32_t b_lo0 = (1u << 16) | (w_smem >> 4);              // LBO(=1) | start address, 16-byte units
-      const uint32_t b_hi = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO | version | SWIZZLE_128B
-      MmaLoopArgs g;
-      g.bar_tfull = bar_tfull;
-      g.bar_tempty = bar_tempty;
-      g.bar_afull = bar_afull;
-      g.bar_aempty = bar_aempty;
-      g.tmem_base = tmem_base;
-      g.a_base = (1u << 16) | (a_smem >> 4);
-      g.b_lo0 = b_lo0;
-      g.b_hi = b_hi;
-      g.ntiles = my_tiles;
-      g.S = (uint32_t)S;
-      g.commit_stage = !res_smem;
-      const uint32_t which = (warp == kMmaWarp) ? 0u : 1u;
-      // Two issuers lift the MMA-only floor (ablation, block-3 ResConv: 2445 -> 2154 cycles per tile) but not the whole
-      // kernel (3397 vs 3686: more contention with the epilogue warps on the same schedulers), so one is the default;
-      // p.issuers = 2 (VFI_ISSUERS=2) keeps the other path measurable.
-      const uint32_t nissuers = (!PAIR && p.issuers == 2 && !RING && (S & 1) == 0) ? 2u : 1u;
-      if (which >= nissuers) g.ntiles = 0;
-      if (RING) {
-        mma_tile_loop<9, 4, true, PAIR>(p, g, which, nissuers);
-      } else {
-        switch (p.nruns * 8 + p.run_len) {  // fully unrolled issue sequences (tapconv_plan admits only these)
-          case 9 * 8 + 1: mma_tile_loop<9, 1, false, PAIR>(p, g, which, nissuers); break;
-          case 27 * 8 + 1: mma_tile_loop<27, 1, false, PAIR>(p, g, which, nissuers); break;
-          case 9 * 8 + 2: mma_tile_loop<9, 2, false, PAIR>(p, g, which, nissuers); break;
-          case 27 * 8 + 2: mma_tile_loop<27, 2, false, PAIR>(p, g, which, nissuers); break;
-          case 9 * 8 + 4: mma_tile_loop<9, 4, false, PAIR>(p, g, which, nissuers); break;
-          case 18 * 8 + 4: mma_tile_loop<18, 4, false, PAIR>(p, g, which, nissuers); break;
-          default: mma_tile_loop<27, 4, false, PAIR>(p, g, which, nissuers); break;
-        }
-      }
-    }
-  } else if (warp == kTmaWarp) {
+  if (warp == kTmaWarp) {
     // ======================================================= TMA producer (one thread feeds the whole pipeline)
-    if (elect_one_sync() && !ABLATE(1024)) {
+    if (lane == 0) {
       mbar_arrive_expect_tx(bar_w, p.w_bytes);
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)wslice * p.w_bytes;
+      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_bytes;
       for (uint32_t off = 0; off < p.w_bytes; off += 32768u)
         bulk_g2s(w_smem + off, wsrc + off, min(32768u, p.w_bytes - off), bar_w);
       // weights do not depend on the previous kernel; its output (our input tensor) does
       asm volatile("griddepcontrol.wait;" ::: "memory");
       TileIter it(p, first, tstep);
-      // pair mode: the transaction bytes of BOTH CTAs' window copies are counted on the LEADER's "full" barrier (the
-      // MMA-issuing thread lives there); the leader's producer announces twice the bytes, the follower's nothing
-      const uint32_t full_base = PAIR ? mapa_u32(bar_afull, 0) : bar_afull;
-      const uint32_t expect = PAIR ? 2u * p.tx_bytes : p.tx_bytes;
-      auto load = [&](uint32_t dst, const void* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
-        if (PAIR)
-          tma_load_4d_pair(dst, tm, bar, c0, c1, c2, c3);
-        else
-          tma_load_4d(dst, tm, bar, c0, c1, c2, c3);
-      };
-      if (RING) {
-        uint32_t slot = 0, ph = 0;
-        for (int k = 0; k < my_tiles; ++k, it.next()) {
-          const int gy0 = it.ty * kTileH + p.halo_y0, gx0 = it.tx * kTileW + p.halo_x0;
+      uint32_t stage = 0, eph = 1;  // window stage / ring slot and the parity of its "empty" barrier
+      for (int k = 0; k < my_tiles; ++k, it.next()) {
+        const int gy0 = it.ty * kTileH + p.halo_y0, gx0 = it.tx * kTileW + p.halo_x0;
+        if (RING) {
           for (int kb = 0; kb < p.nkb; ++kb) {
-            mbar_wait(bar_aempty + 8 * slot, ph ^ 1u, 4);
-            if (rank == 0) mbar_arrive_expect_tx(bar_afull + 8 * slot, expect);
-            load(a_smem + slot * p.stage_bytes, &p.tm64, full_base + 8 * slot, kb * 64, gx0, gy0, it.b);
-            if (++slot == (uint32_t)S) {
-              slot = 0;
-              ph ^= 1u;
+            const uint32_t full = bar_afull + 16 * stage + 8 * (k & 1);  // tile k goes to warpgroup k % 2
+            mbar_wait(bar_aempty + 8 * stage, eph);
+            mbar_arrive_expect_tx(full, p.tx_bytes);
+            tma_load_4d(a_smem + stage * p.stage_bytes, &p.tm64, full, kb * 64, gx0, gy0, it.b);
+            if (++stage == (uint32_t)S) {
+              stage = 0;
+              eph ^= 1u;
             }
           }
-        }
-      } else {
-      uint32_t stage = 0, eph = 1;  // window stage and the parity of its "empty" barrier
-      for (int k = 0; k < my_tiles; ++k, it.next()) {
-        const int b = it.b;
-        const int gy0 = it.ty * kTileH + p.halo_y0, gx0 = it.tx * kTileW + p.halo_x0;
-        mbar_wait(bar_aempty + 8 * stage, eph, 4);
-        if (ABLATE(8)) {
-          if (rank == 0) mbar_arrive(bar_afull + 8 * stage);
         } else {
-          if (rank == 0) mbar_arrive_expect_tx(bar_afull + 8 * stage, expect);
+          const uint32_t full = bar_afull + 16 * stage + 8 * (k & 1);
+          mbar_wait(bar_aempty + 8 * stage, eph);
+          mbar_arrive_expect_tx(full, p.tx_bytes);
           const uint32_t dst = a_smem + stage * p.stage_bytes;
           for (int kb = 0; kb < p.nkb; ++kb) {
             const bool tail = has_tail && (kb == p.nkb - 1);
-            load(dst + p.kb_off[kb], tail ? &p.tm32 : &p.tm64, full_base + 8 * stage, kb * 64, gx0, gy0, b);
+            tma_load_4d(dst + p.kb_off[kb], tail ? &p.tm32 : &p.tm64, full, kb * 64, gx0, gy0, it.b);
           }
-        }
-        if (++stage == (uint32_t)S) {
-          stage = 0;
-          eph ^= 1u;
-        }
-      }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ======================================================= epilogue (warps 0..15)
-    // Four groups of four warps (TMEM lane quarters); group g takes the CTA's tiles g, g + 4, ... and with them TMEM
-    // accumulator g: the issuing thread can run up to three tiles ahead of any group, and a tile's fixed costs (tile
-    // walk, barrier waits, address arithmetic) are paid by four warps instead of eight.
-    const int q = warp & 3;                    // TMEM lane quarter this warp may read
-    const uint32_t acc = (uint32_t)warp >> 2;  // group == TMEM accumulator == tile index mod 4
-    float* ss = reinterpret_cast<float*>(smem + p.off_ss);  // per-channel shift of this CTA's output slice
-    for (int i = threadIdx.x; i < p.n_epi; i += 32 * kEpiWarps) ss[i] = p.shift[n0 + i];
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
-    // the previous kernel may still be reading the buffer we store to (ping-pong) and ring layers read the residual from
-    // global memory: every storing / loading thread orders itself after the previous grid
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-
-    const int r = q * 32 + lane;  // accumulator row == TMEM lane == tile cell
-    const int py = r >> 3, px = r & 7;
-    const uint32_t center_px = (uint32_t)((py - p.halo_y0) * p.halo_w + (px - p.halo_x0));
-    const int nchunks = p.n_epi >> 4;  // 16-column chunks of this CTA's accumulator (<= 8)
-    // "accumulator drained": the issuing thread (pair mode: in the leader CTA) waits for the groups of both CTAs
-    auto release_acc = [&](uint32_t a) {
-      if (PAIR && rank != 0)
-        mbar_arrive_remote(mapa_u32(bar_tempty + 8 * a, 0));
-      else
-        mbar_arrive(bar_tempty + 8 * a);
-    };
-    // stage_out (n_cta == 64, plain NHWC output): this group's tile goes to its own 16 KB staging buffer in the
-    // SWIZZLE_128B form (row = cell, 128 B = the 64 channels) and leaves with one TMA tensor store.  ncu r01_v12: the
-    // direct stores - every lane of an STG.128 in a different 128-byte line - were 2048 L1 tag lookups per tile, 60 %
-    // of the L1/shared data-pipe traffic of a kernel whose tensor-core operands come through the same pipe.
-    const bool stage_out = !LAST && p.stage_out != 0;
-    uint8_t* stg = smem + p.off_stg + acc * (128u * 128u);
-    const uint32_t stg_u32 = smem_base + p.off_stg + acc * (128u * 128u);
-    const bool stg_leader = (q == 0) && (lane == 0);  // issues and tracks this group's bulk stores
-    const float slope = (p.epi_mode == EPI_BIAS) ? 1.f : 0.2f;  // max(a, slope * a): LeakyReLU(0.2), or no activation
-
-    // this group's tiles: k = acc, acc + 4, ... (k counts the CTA's tiles); window stage of tile k = k % S, carried
-    // incrementally together with its use count (parity of the "full" barrier)
-    uint32_t k = acc;
-    uint32_t stage = acc % (uint32_t)S, use = acc / (uint32_t)S;
-    if (ABLATE(1024)) k = 0x7fffffffu;
-    TileIter it(p, first + (int)acc * tstep, kAccBufs * tstep);
-    for (; k < (uint32_t)my_tiles; k += kAccBufs, it.next()) {
-      if (k != acc) {  // advance (stage, use) by kAccBufs tiles
-        stage += kAccBufs;
-        while (stage >= (uint32_t)S) {
-          stage -= (uint32_t)S;
-          ++use;
-        }
-      }
-      const uint32_t vuse = k / kAccBufs;
-      const int b = it.b;
-      const int gy = it.ty * kTileH + py, gx = it.tx * kTileW + px;
-      const bool valid = (gy < p.H) && (gx < p.W) && (b < p.B);  // (b == B: the dummy tile of an odd tile count)
-
-      mbar_wait(bar_tfull + 8 * acc, vuse & 1, 5);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * p.acc_stride + ((uint32_t)(q * 32) << 16);
-
-      if (LAST) {
-        // accumulator column n = c5*16 + pos: component c5 (4 flow + mask) of sub-pixel pos = y4*4 + x4 of the 4x4
-        // patch of this feature cell; two rounds of 8 positions (patch rows 0-1, then 2-3)
-        const int ncomp = nchunks;  // 5 (all components in this CTA) or 1 (component = split)
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t v[5][8];
-#pragma unroll
-          for (int c = 0; c < 5; ++c)
-            if (c < ncomp) tmem_ld8(taddr + c * 16 + half * 8, v[c]);
-          tmem_ld_wait();
-          if (half == 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release_acc(acc);  // TMEM buffer free again
+          if (++stage == (uint32_t)S) {
+            stage = 0;
+            eph ^= 1u;
           }
-          if (valid) {
-            const int Hs = p.H * 4, Ws = p.W * 4;
-#pragma unroll
-            for (int yy = 0; yy < 2; ++yy) {
-              const size_t o = ((size_t)b * Hs + (gy * 4 + half * 2 + yy)) * Ws + gx * 4;
-              if (ncomp == 5 && p.st256) {
-                // the four pixels of this patch row are contiguous: 64 B of flow = two 32-byte stores, 16 B of mask = one
-                uint32_t fw[16], mw[4];
-#pragma unroll
-                for (int x4 = 0; x4 < 4; ++x4) {
-                  const int i = yy * 4 + x4, pos = half * 8 + i;
-#pragma unroll
-                  for (int c = 0; c < 4; ++c) fw[x4 * 4 + c] = __float_as_uint(__uint_as_float(v[c][i]) + ss[c * 16 + pos]);
-                  mw[x4] = __float_as_uint(__uint_as_float(v[4][i]) + ss[4 * 16 + pos]);
-                }
-                const uint32_t lo[8] = {fw[0], fw[1], fw[2], fw[3], fw[4], fw[5], fw[6], fw[7]};
-                const uint32_t hi[8] = {fw[8], fw[9], fw[10], fw[11], fw[12], fw[13], fw[14], fw[15]};
-                stg256(p.out_flow + o, lo);
-                stg256(p.out_flow + o + 2, hi);
-                *reinterpret_cast<uint4*>(p.out_mask + o) = make_uint4(mw[0], mw[1], mw[2], mw[3]);
-              } else if (ncomp == 5) {
-#pragma unroll
-                for (int x4 = 0; x4 < 4; ++x4) {
-                  const int i = yy * 4 + x4, pos = half * 8 + i;
-                  float4 f;
-                  f.x = __uint_as_float(v[0][i]) + ss[0 * 16 + pos];
-                  f.y = __uint_as_float(v[1][i]) + ss[1 * 16 + pos];
-                  f.z = __uint_as_float(v[2][i]) + ss[2 * 16 + pos];
-                  f.w = __uint_as_float(v[3][i]) + ss[3 * 16 + pos];
-                  p.out_flow[o + x4] = f;
-                  p.out_mask[o + x4] = __uint_as_float(v[4][i]) + ss[4 * 16 + pos];
-                }
-              } else {
-                const int c5 = split;  // output channels split across CTAs (large c): one component per CTA
-#pragma unroll
-                for (int x4 = 0; x4 < 4; ++x4) {
-                  const int i = yy * 4 + x4, pos = half * 8 + i;
-                  const float val = __uint_as_float(v[0][i]) + ss[pos];
-                  if (c5 < 4)
-                    reinterpret_cast<float*>(p.out_flow)[(o + x4) * 4 + c5] = val;
-                  else
-                    p.out_mask[o + x4] = val;
-                }
-              }
-            }
-          }
-        }
-        continue;
-      }
-
-      // ---- conv0.x / ResConv: this thread owns one grid cell and all n_cta channels of it, two 16-channel chunks per
-      // round (at most 32 accumulator values live per thread: 608 threads, 96 registers each)
-      // (patch form, out_s2d == 2: columns are (sub-pixel, channel) pairs, placed per chunk in finish_chunk)
-      const bool patch = (p.out_s2d == 2);
-      T* orow = reinterpret_cast<T*>(p.out) + (valid ? out_pixel_offset(p, b, gy, gx) + (patch ? 0 : (size_t)n0) : 0);
-      if (stage_out) {  // the previous store of this group must have finished reading the staging buffer
-        if (stg_leader) bulk_wait_read0();
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + (int)acc) : "memory");
-      }
-      const uint4* gres = nullptr;  // ring layers: the centre pixel's channels in the input tensor (L2 hit)
-      if (RING && residual)
-        gres = reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(p.in) +
-                                              ((((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.cin + (size_t)n0));
-      const uint32_t st_u32 = smem_base + p.off_a + stage * p.stage_bytes;  // this tile's window (shared-space address)
-      // residual of chunk c = input channels n0 + 16*c .. +15 of the centre pixel: two 16-byte chunks of its swizzled row.
-      // Explicit ld.shared with the per-lane XOR in the address: with plain C++ loads the compiler, seeing all eight
-      // chunk offsets of the row over the unrolled chunk loop, read the row linearly ([base + 16k] for every lane) and
-      // permuted registers afterwards - every lane of an LDS.128 then sits in the same four banks (ncu r01_v14: 6.9 M
-      // bank-conflict wavefronts, 11 per LDS.128 instead of 2.7, in a kernel whose tensor-core operand reads fill 61 %
-      // of the same shared-memory data pipe).  Issued while the tcgen05.ld of the chunk is in flight.
-      auto load_residual = [&](int c, uint4& r0, uint4& r1) {
-        r0 = make_uint4(0u, 0u, 0u, 0u);
-        r1 = r0;
-        if (res_smem && !ABLATE(1)) {
-          const int ch0 = n0 + c * 16;
-          const int kb = ch0 >> 6;
-          const bool tail = has_tail && (kb == p.nkb - 1);
-          // stage base and k-block offsets are multiples of 1024, so the swizzle phase of the row depends only on the
-          // pixel: (address >> 7) & 7 for 128-byte rows, & 3 for the 64-byte rows of a 32-channel tail
-          const uint32_t row = p.kb_off[kb] + (tail ? center_px * 64u : center_px * 128u);
-          const uint32_t c0 = (uint32_t)(ch0 - kb * 64) >> 3, sw = tail ? ((center_px >> 1) & 3u) : (center_px & 7u);
-          r0 = lds128(st_u32 + row + ((c0 ^ sw) << 4));
-          r1 = lds128(st_u32 + row + (((c0 + 1u) ^ sw) << 4));
-        } else if (RING && residual && valid) {
-          r0 = __ldg(gres + c * 2);
-          r1 = __ldg(gres + c * 2 + 1);
-        }
-      };
-      auto finish_chunk = [&](int c, const uint32_t(&vv)[16], const uint4 r0, const uint4 r1) {
-        const float4* sp = reinterpret_cast<const float4*>(ss + c * 16);
-        const float4 s0 = sp[0], s1 = sp[1], s2 = sp[2], s3 = sp[3];
-        const float shf[16] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w,
-                               s2.x, s2.y, s2.z, s2.w, s3.x, s3.y, s3.z, s3.w};
-        const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-        uint32_t o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float a0 = __uint_as_float(vv[2 * j]) + shf[2 * j];
-          float a1 = __uint_as_float(vv[2 * j + 1]) + shf[2 * j + 1];
-          if (residual) {
-            const float2 rf = Pack2<T>::unpack(rw[j]);
-            a0 += rf.x;
-            a1 += rf.y;
-          }
-          o[j] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));  // LeakyReLU(0.2) / identity
-        }
-        if (stage_out) {  // chunks 2c, 2c+1 of row r, XOR-swizzled with (r & 7) like every SWIZZLE_128B tile
-          uint8_t* rowp = stg + (uint32_t)r * 128u;
-          *reinterpret_cast<uint4*>(rowp + (((uint32_t)(2 * c) ^ ((uint32_t)r & 7u)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<uint4*>(rowp + (((uint32_t)(2 * c + 1) ^ ((uint32_t)r & 7u)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-          return;
-        }
-        // 32 contiguous bytes (16 channels) of this cell's channel vector; L2 merges the halves of a sector
-        if (valid && (!ABLATE(1) || o[0] == 0x12345678u)) {
-          uint4* dst = reinterpret_cast<uint4*>(orow + c * 16);
-          if (patch) {  // 16 columns = sub-pixels pos0, pos0 + 1 (same patch row, adjacent x) x 8 channels: 32 contiguous bytes
-            const int pos0 = (n0 + c * 16) >> 3;
-            dst = reinterpret_cast<uint4*>(orow + ((size_t)(pos0 >> 2) * (size_t)(4 * p.W) + (size_t)(pos0 & 3)) * 8);
-          }
-          if (p.st256)
-            stg256(dst, o);
-          else {
-            dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
-            dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
-          }
-        }
-      };
-      if (ABLATE(4)) {
-        __syncwarp();
-        if (lane == 0) release_acc(acc);
-        if (res_smem && lane == 0) mbar_arrive(bar_aempty + 8 * stage);
-        continue;
-      }
-      // acquire the TMA-written window.  (The follower CTA of a pair has no "full" barrier of its own - its copies are
-      // counted on the leader's - and is ordered behind them through the MMAs that read the window and their commit
-      // on t_full, which it has just waited for.)
-      if (res_smem && !(PAIR && rank != 0)) mbar_wait(bar_afull + 8 * stage, use & 1, 6);
-      for (int c = 0; c < nchunks; c += 2) {
-        uint32_t v0[16], v1[16];
-        const bool two = (c + 1 < nchunks);
-        tmem_ld16(taddr + c * 16, v0);
-        if (two) tmem_ld16(taddr + (c + 1) * 16, v1);
-        uint4 ra0, ra1, rb0, rb1;
-        load_residual(c, ra0, ra1);
-        if (two) load_residual(c + 1, rb0, rb1);
-        tmem_ld_wait();
-        if (c + 2 >= nchunks) {  // last round: the accumulator has been read completely
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) release_acc(acc);  // TMEM buffer free: its next tile's MMAs may start
-        }
-        if (ABLATE(2)) {
-          if (v0[0] == 0x12345678u && v1[1] == 0x9abcdef0u) reinterpret_cast<T*>(p.out)[0] = T(1.f);  // keep the loads
-          continue;
-        }
-        finish_chunk(c, v0, ra0, ra1);
-        if (two) finish_chunk(c + 1, v1, rb0, rb1);
-      }
-      if (res_smem) {
-        // our generic-proxy READS of the window are complete (values consumed above); the mbarrier arrive/wait pair
-        // orders them before the producer's next TMA write - no generic write is involved, so no proxy fence
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);
-      }
-      if (stage_out) {
-        fence_proxy_async();  // this thread's staging writes -> visible to the TMA (async proxy)
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + (int)acc) : "memory");
-        if (stg_leader && b < p.B) {
-          tma_store_4d(&p.tm_out, stg_u32, n0, it.tx * kTileW, it.ty * kTileH, b);
-          bulk_commit_group();
         }
       }
     }
-    if (stage_out && stg_leader) bulk_wait0();  // the stores are performed before the grid counts as complete
+    return;
   }
 
-  tc_fence_before();
-  if (PAIR)
-    cluster_sync_all();  // neither CTA may leave (or free TMEM) while the pair's MMAs, commits or remote arrives are in flight
-  else
-    __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    if (PAIR)
-      tmem_dealloc_pair(tmem_base, p.tmem_cols);
-    else
-      tmem_dealloc(tmem_base, p.tmem_cols);
+  // ========================================================= MMA + epilogue warpgroups
+  // Warpgroup g consumes the stages of tiles g, g + 2, ... through its own "full" barrier of each stage: the fills a
+  // warpgroup waits for on one barrier are its own, in order, so a parity wait never confuses an older phase with the
+  // one it wants (a stage shared by both warpgroups would, with one or an odd number of stages).
+  const int g = warp >> 2;
+  const int wq = warp & 3;  // warp of the warpgroup: rows 16 wq .. 16 wq + 15 of each 64-row half
+  // the previous kernel may still be reading the buffer we store to (ping-pong) and ResConv layers read the residual
+  // from global memory: every storing / loading thread orders itself after the previous grid
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  mbar_wait(bar_w, 0);
+  const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);  // LBO(=1) | start address, 16-byte units
+  const uint32_t b_lo0 = (1u << 16) | (w_smem >> 4);
+  const uint32_t per_tile = RING ? (uint32_t)p.nkb : 1u;  // stages / slots one tile consumes
+  const uint32_t b_kb = (9u * (uint32_t)p.n_cta * 128u) >> 4;  // ring: weight bytes of one k-block, 16-byte units
+  const uint32_t stage_units = p.stage_bytes >> 4;
+  uint32_t stage = 0, ph_bits = 0;  // window stage / ring slot; bit s: parity of this warpgroup's next wait on stage s
+  auto advance = [&](uint32_t n) {
+    stage += n;
+    while (stage >= (uint32_t)S) stage -= (uint32_t)S;
+  };
+  auto wait_full = [&]() {
+    mbar_wait(bar_afull + 16 * stage + 8 * (uint32_t)g, (ph_bits >> stage) & 1u);
+    ph_bits ^= 1u << stage;
+  };
+  advance((uint32_t)g * per_tile);
+  const float slope = (p.epi_mode == EPI_BIAS) ? 1.f : 0.2f;  // max(a, slope * a): LeakyReLU(0.2), or no activation
+  const int px = lane >> 2;             // tile column of this thread's accumulator rows
+  const int c2 = 2 * (lane & 3);        // first of this thread's two columns in every 8-column block
+  float acc[2][N / 2];
+
+  TileIter it(p, first + g * tstep, kMmaGroups * tstep);
+  for (int k = g; k < my_tiles; k += kMmaGroups, it.next()) {
+    if (RING) {
+      uint32_t prev = 0;
+      for (int kb = 0; kb < p.nkb; ++kb) {
+        wait_full();
+        wgmma_fence();
+        issue_window<N, T>(p, acc, a_lo0 + stage * stage_units, b_lo0 + (uint32_t)kb * b_kb, kb > 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) {  // the previous slot's MMAs have read it
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_aempty + 8 * prev);
+        }
+        prev = stage;
+        advance(1u);
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_aempty + 8 * prev);
+      advance(per_tile);  // the other warpgroup's tile
+    } else {
+      wait_full();
+      wgmma_fence();
+      issue_window<N, T>(p, acc, a_lo0 + stage * stage_units, b_lo0, 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);  // window free once the MMAs have read it
+      advance((uint32_t)kMmaGroups);
+    }
+    acc_fence(acc[0]);
+    acc_fence(acc[1]);
+
+    // ---- epilogue straight from the accumulator registers: d[h][4 j + 2 e + c] = tile row 8 h + 2 wq + e, column
+    // 8 j + c2 + c
+    const int b = it.b;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int gy = it.ty * kTileH + 8 * h + 2 * wq + e, gx = it.tx * kTileW + px;
+        if (gy >= p.H || gx >= p.W) continue;
+        if (LAST) {
+          // column n = c5*16 + pos: component c5 (4 flow + mask) of sub-pixel pos = y4*4 + x4 of this cell's 4x4 patch
+          const int Hs = p.H * 4, Ws = p.W * 4;
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) {
+            const int n = n0 + 8 * j + c2;
+            const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + n));
+            const int c5 = n >> 4, pos = n & 15;  // n even: n + 1 is the next sub-pixel of the same patch row
+            const size_t o = ((size_t)b * Hs + (gy * 4 + (pos >> 2))) * Ws + gx * 4 + (pos & 3);
+            const float v0 = acc[h][4 * j + 2 * e] + sh.x, v1 = acc[h][4 * j + 2 * e + 1] + sh.y;
+            if (c5 < 4) {
+              float* f = reinterpret_cast<float*>(p.out_flow + o);
+              f[c5] = v0;
+              f[4 + c5] = v1;
+            } else {
+              *reinterpret_cast<float2*>(p.out_mask + o) = make_float2(v0, v1);
+            }
+          }
+        } else {
+          const bool patch = (p.out_s2d == 2);
+          T* orow = reinterpret_cast<T*>(p.out) + out_pixel_offset(p, b, gy, gx);
+          const T* rrow = reinterpret_cast<const T*>(p.in) + (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.cin;
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) {
+            const int n = n0 + 8 * j + c2;
+            const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + n));
+            float a0 = acc[h][4 * j + 2 * e] + sh.x, a1 = acc[h][4 * j + 2 * e + 1] + sh.y;
+            if (residual) {
+              const float2 rf = Pack2<T>::unpack(__ldg(reinterpret_cast<const unsigned int*>(rrow + n)));
+              a0 += rf.x;
+              a1 += rf.y;
+            }
+            // patch form: columns n = sub-pixel (n >> 3) x channel (n & 7)
+            const size_t off = patch ? ((size_t)((n >> 3) >> 2) * (size_t)(4 * p.W) + (size_t)((n >> 3) & 3)) * 8 + (n & 7)
+                                     : (size_t)n;
+            *reinterpret_cast<uint32_t*>(orow + off) = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+          }
+        }
+      }
   }
 }
 
@@ -788,13 +438,10 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   // input window: one 1024-aligned region per k-block (64 channels = 128-byte rows; 32-channel tail = 64-byte rows)
   p.nkb = (L.cin + 63) / 64;
   p.ring = L.ring;
-  p.pair = L.pair;
-  p.n_epi = L.pair ? 2 * L.n_cta : L.n_cta;
   if (L.ktotal16 > kMaxK16) return 0;
-  // n_cta rows of B per CTA (whole 8-row swizzle atoms); n_epi accumulator columns: a multiple of 16 (the MMA's N for
-  // M = 128 / 256 and the epilogue's chunk), four accumulators of at most 128 columns in the 512 TMEM columns
-  if (p.nkb > kMaxKBlocks || L.n_cta > 96 || (L.n_cta & 7) || (p.n_epi & 15) || p.n_epi > 128) return 0;
-  if (L.pair && (L.nsplit & 1)) return 0;
+  // n_cta = the wgmma N: whole 8-row swizzle atoms of B, and a multiple of 16 with an instantiated kernel (<= 96: two
+  // 64-row accumulators of n_cta fp32 columns per thread)
+  if (p.nkb > kMaxKBlocks || L.n_cta > 96 || (L.n_cta & 15) || L.n_cta < 16) return 0;
   if (L.ring && ((L.cin & 63) || L.ntaps != 9 * p.nkb || L.ktotal16 != 36 * p.nkb)) return 0;
   uint32_t off = 0;
   p.tx_bytes = 0;
@@ -815,8 +462,8 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   }
   p.stage_bytes = off;
   {
-    // descriptor words per K=16 step (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14) | LBO [16,30) ; SBO>>4 [32,46) |
-    // version=1 [46,48) | layout [61,64) (2 = SWIZZLE_128B, 4 = SWIZZLE_64B); base_offset stays 0.
+    // wgmma descriptor words per K=16 step (ptx.cuh): start>>4 [0,14) | LBO [16,30) ; SBO>>4 [32,46) | layout [62,64)
+    // (1 = SWIZZLE_128B, 2 = SWIZZLE_64B); base_offset stays 0.
     // Ring layers list their taps k-block-major, so entries [0,36) (k-block 0) serve every k-block: the kernel adds
     // the slot address to A and kb * (9 * n_cta * 128 B) to B.
     uint4 step[kMaxK16];
@@ -831,7 +478,7 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
         const uint32_t a_off = p.kb_off[kb] + (uint32_t)((te.dy - L.halo_y0) * L.halo_w + (te.dx - L.halo_x0)) * rowb +
                                (uint32_t)(ch0 - kb * 64) * 2u;
         const uint32_t b_off = (uint32_t)(j >> 2) * ((uint32_t)L.n_cta * 128u) + (uint32_t)(j & 3) * 32u;
-        step[j] = make_uint4(a_off >> 4, (((uint32_t)L.halo_w * rowb) >> 4) | (1u << 14) | ((tail ? 4u : 2u) << 29),
+        step[j] = make_uint4(a_off >> 4, (((uint32_t)L.halo_w * rowb) >> 4) | (tail ? kDescSw64 : kDescSw128),
                              b_off >> 4, 0u);
       }
     // group the steps into runs of run_len = 4, 2 or 1 whose descriptors advance by 32 B (2 units) per step
@@ -850,55 +497,20 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
     }
     p.run_len = run_len;
     p.nruns = nsteps / run_len;
-    {
-      const int key = p.nruns * 8 + run_len;  // the issue sequences the kernel has
-      const bool have = key == 9 * 8 + 1 || key == 27 * 8 + 1 || key == 9 * 8 + 2 || key == 27 * 8 + 2 ||
-                        key == 9 * 8 + 4 || key == 18 * 8 + 4 || key == 27 * 8 + 4;
-      if (!have || (L.ring && key != 9 * 8 + 4)) return 0;
-    }
     for (int r = 0; r < p.nruns; ++r) p.mma[r] = step[r * run_len];
   }
-  p.off_ss = kCtrlBytes;
-  p.off_w = align_up(p.off_ss + (uint32_t)p.n_epi * 4u, 1024);
+  p.b_hi = (1024u >> 4) | kDescSw128;  // B: SBO = 8 rows x 128 B, SWIZZLE_128B
+  p.off_w = align_up(kCtrlBytes, 1024);
   p.off_a = align_up(p.off_w + p.w_bytes, 1024);
-  // staged output (TMA tensor store): 64-channel slices of a plain NHWC output, when four 16 KB staging buffers still
-  // leave room for three window stages
-  static const int opt_store = [] {  // VFI_STORE: 0 = two STG.128 per chunk, 1 = one STG.256, 2 = 1 + staged TMA store
-    const char* e = std::getenv("VFI_STORE");
-    return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : kDefaultStoreMode;
-  }();
-  p.st256 = opt_store >= 1;
-  const uint32_t stg_bytes = (uint32_t)kAccBufs * 128u * 128u;
-  // (r01_v13, block 3 at batch 8: conv0.1 84.8 -> 69.7 us with the staged store; the ResConv layers, whose window
-  // stages are held until the epilogue has read the residual, lost more from the fourth stage than they gained:
-  // 94.2 us with STG.256 and 4 stages, 109 us staged with 3 - so only layers without a residual stage their output)
-  p.stage_out = (opt_store >= 2 && p.n_epi == 64 && L.out_s2d == 0 && !L.ring &&
-                 (L.epi_mode == EPI_BIAS_LRELU || L.epi_mode == EPI_BIAS) &&
-                 p.off_a + 3u * p.stage_bytes + stg_bytes <= (uint32_t)kSmemLimit)
-                    ? 1 : 0;
-  static const int max_stages = [] {
-    const char* e = std::getenv("VFI_STAGES_MAX");
-    return (e && e[0] >= '1' && e[0] <= '6') ? e[0] - '0' : kDefaultMaxStages;
-  }();
-  const uint32_t limit = (uint32_t)kSmemLimit - (p.stage_out ? stg_bytes : 0u);
   int stages = 0;
-  // ResConv layers hold a window stage until the epilogue - up to three tiles behind the MMAs - has read the residual
-  // from it, so they take up to six stages (r01_v14, block 3 at batch 8: 93.2 -> 87.8 -> 82.9 us with 4 / 5 / 6)
-  const int cap = L.ring ? kMaxStages : (L.epi_mode == EPI_RESCONV ? kMaxStages : max_stages);
-  for (int s = cap; s >= 1; --s) {
-    if (p.off_a + (uint32_t)s * p.stage_bytes <= limit) {
+  for (int s = kMaxStages; s >= 1; --s) {
+    if (p.off_a + (uint32_t)s * p.stage_bytes <= (uint32_t)kSmemLimit) {
       stages = s;
       break;
     }
   }
   p.stages = stages;
-  p.off_stg = p.off_a + (uint32_t)stages * p.stage_bytes;  // stage sizes are multiples of 1024
-  p.smem_bytes = p.off_stg + (p.stage_out ? stg_bytes : 0u);
-  // accumulators: kAccBufs buffers of n_cta fp32 columns, allocation is a power of two >= 32 (<= 4 x 128 = 512)
-  uint32_t stride = 16;
-  while (stride < (uint32_t)p.n_epi) stride <<= 1;
-  p.acc_stride = stride;
-  p.tmem_cols = stride * kAccBufs < 32 ? 32 : stride * kAccBufs;
+  p.smem_bytes = p.off_a + (uint32_t)stages * p.stage_bytes;  // stage sizes are multiples of 1024
   return stages;
 }
 
@@ -913,19 +525,6 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     set_error("tapconv: space-to-depth output needs even H and W");
     return cudaErrorInvalidValue;
   }
-  {
-    static const int issuers = [] {
-      const char* e = std::getenv("VFI_ISSUERS");
-      return (e && e[0] == '2') ? 2 : 1;
-    }();
-    p.issuers = issuers;
-  }
-#ifdef VFI_ABLATE
-  {
-    const char* e = std::getenv("VFI_ABLATE");
-    p.ablate = e ? std::atoi(e) : 0;
-  }
-#endif
   p.in = in;
   p.out = out;
   p.out_flow = out_flow;
@@ -938,10 +537,6 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
   p.tiles_y = (H + kTileH - 1) / kTileH;
   p.tiles_x = (W + kTileW - 1) / kTileW;
   p.ntiles = B * p.tiles_y * p.tiles_x;
-  // instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): D=f32, A/B = f16|bf16, both K-major,
-  // N>>3 at [17,23), M>>4 at [24,29)
-  const uint32_t fmt = (op_type == OP_BF16) ? 1u : 0u;
-  p.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(p.n_epi >> 3) << 17) | (((L.pair ? 256u : 128u) >> 4) << 24);
 
 #ifdef VFI_HOST_EMU
   use_ref = true;  // the host emulation has only the checker kernel
@@ -969,17 +564,12 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
   } else {
     p.tm32 = p.tm64;
   }
-  if (p.stage_out &&
-      !make_tmap(&p.tm_out, dt, out, L.n_total, W, H, B, 64, kTileW, kTileH, CU_TENSOR_MAP_SWIZZLE_128B))
-    return cudaErrorInvalidValue;
-  // single CTAs: cps persistent CTAs per output-channel split; pairs: cps PAIRS (= TPCs) per pair-split
-  const int nsplit_u = L.pair ? L.nsplit / 2 : L.nsplit;
-  const int nunits = L.pair ? (p.ntiles + 1) / 2 : p.ntiles;
-  int cps = (L.pair ? num_sms / 2 : num_sms) / nsplit_u;
+  // cps persistent CTAs per output-channel split
+  int cps = num_sms / L.nsplit;
   if (cps < 1) cps = 1;
-  if (cps > nunits) cps = nunits;
+  if (cps > p.ntiles) cps = p.ntiles;
   p.ctas_per_split = cps;
-  const int grid = cps * nsplit_u * (L.pair ? 2 : 1);
+  const int grid = cps * L.nsplit;
   cudaError_t err;  // (per device: set on every launch, it is a cheap driver call)
   static const bool pdl = [] {  // VFI_PDL=0: plain stream-ordered launches (A/B runs)
     const char* e = std::getenv("VFI_PDL");
@@ -993,15 +583,8 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     cfg.blockDim = dim3((unsigned)kThreads);
     cfg.dynamicSmemBytes = p.smem_bytes;
     cfg.stream = st;
-    cudaLaunchAttribute attr[2];
+    cudaLaunchAttribute attr[1];
     int na = 0;
-    if (L.pair) {  // the two CTAs of a pair are a cluster: co-scheduled on the two SMs of one TPC
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = 2;
-      attr[na].val.clusterDim.y = 1;
-      attr[na].val.clusterDim.z = 1;
-      ++na;
-    }
     if (pdl) {
       attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       attr[na].val.programmaticStreamSerializationAllowed = 1;
@@ -1012,19 +595,23 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     return cudaLaunchKernelEx(&cfg, kern, p);
   };
   const bool last = (L.epi_mode == EPI_LASTCONV);
-  auto pick = [&](auto tag) -> cudaError_t {
+  auto pick_n = [&](auto tag, auto ring, auto lst) -> cudaError_t {
     using T = decltype(tag);
-    const int key = (L.ring ? 4 : 0) | (last ? 2 : 0) | (L.pair ? 1 : 0);
-    switch (key) {
-      case 0: return go(tapconv_kernel<T, false, false, false>);
-      case 1: return go(tapconv_kernel<T, false, false, true>);
-      case 2: return go(tapconv_kernel<T, false, true, false>);
-      case 3: return go(tapconv_kernel<T, false, true, true>);
-      case 4: return go(tapconv_kernel<T, true, false, false>);
-      case 5: return go(tapconv_kernel<T, true, false, true>);
-      case 6: return go(tapconv_kernel<T, true, true, false>);
-      default: return go(tapconv_kernel<T, true, true, true>);
+    constexpr bool R = decltype(ring)::value, LA = decltype(lst)::value;
+    switch (L.n_cta) {  // tapconv_plan admits multiples of 16 up to 96
+      case 16: return go(tapconv_kernel<T, R, LA, 16>);
+      case 32: return go(tapconv_kernel<T, R, LA, 32>);
+      case 48: return go(tapconv_kernel<T, R, LA, 48>);
+      case 64: return go(tapconv_kernel<T, R, LA, 64>);
+      case 80: return go(tapconv_kernel<T, R, LA, 80>);
+      default: return go(tapconv_kernel<T, R, LA, 96>);
     }
+  };
+  auto pick = [&](auto tag) -> cudaError_t {
+    using F = std::false_type;
+    using Tr = std::true_type;
+    if (L.ring) return last ? pick_n(tag, Tr{}, Tr{}) : pick_n(tag, Tr{}, F{});
+    return last ? pick_n(tag, F{}, Tr{}) : pick_n(tag, F{}, F{});
   };
   err = (op_type == OP_BF16) ? pick(__nv_bfloat16{}) : pick(__half{});
   if (err != cudaSuccess) return err;

@@ -41,8 +41,8 @@ struct TapEntry {
 };
 
 constexpr int kMaxTaps = 27;  // 9 taps, or 9 taps x 3 k-blocks in k-block-major (ring) order
-constexpr int kTileH = 16, kTileW = 8;        // one CTA tile = 128 grid cells = UMMA M
-constexpr int kSmemLimit = 232448;            // 227 KB opt-in maximum per CTA on sm_100
+constexpr int kTileH = 16, kTileW = 8;        // one CTA tile = 128 grid cells = two m64 wgmma row blocks
+constexpr int kSmemLimit = 232448;            // 227 KB opt-in maximum per CTA on sm_90
 
 constexpr int kMaxKBlocks = 6;
 constexpr int kMaxK16 = 108;   // 9 taps x 192/16
@@ -50,7 +50,6 @@ constexpr int kMaxK16 = 108;   // 9 taps x 192/16
 struct alignas(64) TapConvParams {
   CUtensorMap tm64;      // input as a {C, W, H, B} tensor with a {64 ch, halo_w, halo_h, 1} box, SWIZZLE_128B
   CUtensorMap tm32;      // same with a {32 ch, ...} box, SWIZZLE_64B (only used when cin % 64 == 32)
-  CUtensorMap tm_out;    // stage_out: the output as a {n_total, W, H, B} tensor with a {64 ch, 8, 16, 1} box, SWIZZLE_128B
   const void* in;        // [B, H, W, cin] 16-bit, NHWC
   void* out;             // [B, H, W, n_total] 16-bit NHWC; out_s2d = 1: its space-to-depth form; out_s2d = 2: the 4x4
                          // sub-pixel patch form [B, 4H, 4W, 8] with column n = (py*4 + px)*8 + ch (arch 4.26 lastconv features)
@@ -65,29 +64,18 @@ struct alignas(64) TapConvParams {
   int stages;
   int epi_mode, out_s2d;
   int nruns, run_len;    // MMA issue: nruns runs of run_len consecutive K=16 steps (mma[r] = first step of run r)
-  int issuers;           // MMA-issuing threads: 1 (default) or 2 (even stage counts only; VFI_ISSUERS=2)
-  int ablate;            // diagnostic builds only (-DVFI_ABLATE): pipeline parts switched off, see tapconv.cu
   int ring;              // 1: the window streams through a ring of single k-block slots (see tapconv.cu)
-  int pair;              // 1: CTA pairs (cluster of 2, tcgen05 cta_group::2): one M = 256 MMA over two tiles, each CTA
-                         //    holding n_cta = n_epi / 2 rows of the B operand; ctas_per_split counts PAIRS
-  int n_epi;             // accumulator columns of a CTA = output channels its epilogue writes (n_cta, pair: 2 * n_cta)
   int tiles_x, tiles_y, ntiles;
   int ctas_per_split;
-  uint32_t idesc;
-  uint32_t tmem_cols, acc_stride;
+  uint32_t b_hi;                  // high word of the weight (B) descriptors
   uint32_t w_bytes;               // packed weight bytes of one split
-  uint32_t off_ss, off_w, off_a, stage_bytes, smem_bytes;
+  uint32_t off_w, off_a, stage_bytes, smem_bytes;
   int nkb;                        // k-blocks of the staged window: 64 channels each, 32-channel tail if cin%64==32
   uint32_t kb_off[kMaxKBlocks];   // byte offset of each k-block inside a stage (1024-aligned)
   uint32_t tx_bytes;              // bytes one stage fill delivers (mbarrier transaction count)
-  int st256;                      // 1: 32-byte STG.256 epilogue stores (one L1 tag lookup per lane and chunk instead of two)
-  int stage_out;                  // 1: the epilogue writes each tile to a shared-memory staging buffer (one per
-                                  //    accumulator group) and ONE TMA tensor store moves it out (n_cta == 64 only)
-  uint32_t off_stg;               // staging buffers: kAccBufs x 128 rows x 128 B, 1024-aligned
   TapEntry taps[kMaxTaps];
   // per run: {A start offset inside a stage, A descriptor high word, B start offset inside the weights, 0},
-  // offsets in 16-byte units.  Lives in the kernel parameters (constant bank) so that the MMA-issuing warp gets it
-  // through uniform loads straight into uniform registers.
+  // offsets in 16-byte units.  Lives in the kernel parameters (constant bank): uniform loads for the MMA warpgroups.
   uint4 mma[kMaxK16];
 };
 
@@ -98,7 +86,6 @@ struct TapConvLayer {
   int halo_y0 = 0, halo_x0 = 0, halo_h = 0, halo_w = 0;
   int epi_mode = 0, out_s2d = 0;
   int ring = 0;           // taps are listed k-block-major (kb, tap) with nk16 = 4; needs cin % 64 == 0
-  int pair = 0;           // CTA pairs: packed slices 2s and 2s+1 (n_cta rows each) are the two halves of pair-split s
   TapEntry taps[kMaxTaps];
   void* w = nullptr;      // device
   float* shift = nullptr; // device
@@ -116,7 +103,7 @@ constexpr int kMaxBatch = 16;
 enum OperandType : int { OP_F16 = 0, OP_BF16 = 1 };
 
 // ---- launchers (defined in tapconv.cu / elementwise.cu) -------------------------------------
-// Returns cudaSuccess or the launch error; `use_ref` runs the CUDA-core checker instead of the tcgen05 kernel.
+// Returns cudaSuccess or the launch error; `use_ref` runs the CUDA-core checker instead of the tensor-core kernel.
 cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, void* out, float4* out_flow,
                            float* out_mask, int B, int H, int W, int num_sms, bool use_ref, cudaStream_t st);
 // smem/stage plan for a layer (for DESIGN.md tables and tests); returns 0 stages when it cannot fit
@@ -208,12 +195,11 @@ struct alignas(64) StreamConvParams {
   int ksize, ntaps, nkb0, nkb;
   int n_total, n_cta, nsplit, act;
   int halo_y0, halo_x0, halo_h, halo_w;
-  int mt, nsets;          // tiles per CTA pass (accumulators sharing a weight slot), accumulator sets (epilogue overlap)
+  int mt;                 // tiles per CTA pass (one per MMA warpgroup, sharing every weight slot)
   int a_slots, b_slots;
   int tiles_x, tiles_y, ntiles, npasses, ctas_per_split;
-  uint32_t idesc, tmem_cols, acc_stride;
   uint32_t a_tx_bytes, a_win_bytes, a_slot_bytes, b_slot_bytes;
-  uint32_t off_ss, off_b, off_a, smem_bytes;
+  uint32_t off_b, off_a, smem_bytes;
   uint32_t a_hi;          // high word of the A descriptors
   uint32_t tap_off[9];    // start-address offset of each tap inside a window, 16-byte units
 };

@@ -53,7 +53,7 @@ def host_copy_frames(frames: torch.Tensor, slots, out: torch.Tensor, threads: in
 
 
 class Rife46Engine:
-    """RIFE 4.6 / 4.7 / 4.17 / 4.26 (rife46.pth; rife47.pth, rife49.pth; rife417.pth; rife426.pth) on one B200.  `state_dict` maps the reference's parameter names to tensors (any float dtype)."""
+    """RIFE 4.6 / 4.7 / 4.17 / 4.26 (rife46.pth; rife47.pth, rife49.pth; rife417.pth; rife426.pth) on one H100.  `state_dict` maps the reference's parameter names to tensors (any float dtype)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, dtype: str = "float32", batch: int = 8,
                  arch: str = None):
@@ -217,7 +217,7 @@ def film_state_dict_names():
 
 
 class FilmEngine:
-    """FILM (film_net_fp32.pt) on one B200: `state_dict` = the TorchScript module's / Interpolator's state_dict."""
+    """FILM (film_net_fp32.pt) on one H100: `state_dict` = the TorchScript module's / Interpolator's state_dict."""
 
     MAX_PAIRS = 16
 
@@ -327,7 +327,7 @@ def sepconv_state_dict_names():
 
 
 class SepconvEngine:
-    """Sepconv (sepconv.pth) on one B200: `state_dict` = sepconv_enhanced.Network's."""
+    """Sepconv (sepconv.pth) on one H100: `state_dict` = sepconv_enhanced.Network's."""
 
     MAX_PAIRS = 16
 

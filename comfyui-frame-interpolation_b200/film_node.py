@@ -1,4 +1,4 @@
-"""ComfyUI node surface of the B200 FILM path: a drop-in for the reference's `FILM VFI` node.
+"""ComfyUI node surface of the H100 FILM path: a drop-in for the reference's `FILM VFI` node.
 
 Mirrors vfi_models/film/__init__.py:12-113: the class attributes and kwargs of ``FILM_VFI``, the bisection
 schedule of ``inference`` (:12-42), the skip semantics (a skipped pair is dropped together with its first

@@ -1,6 +1,6 @@
 """The shared per-pair loop the reference's other nodes (GMFSS, Sepconv, M2M, IFRNet, ...) drive their models through:
 `vfi_utils.generic_frame_loop` / `_generic_frame_loop` (vfi_utils.py:149-389), re-stated for this package so that a
-B200 model function (frame0, frame1, timestep, *args) -> middle frame can be dropped behind any of those nodes.
+H100 model function (frame0, frame1, timestep, *args) -> middle frame can be dropped behind any of those nodes.
 
 Semantics kept (checked against the reference's own outputs, tests/golden/loop_*.npz):
   * int multiplier: every frame is emitted followed by its m-1 middles; a skipped pair keeps its first frame and

@@ -1,4 +1,4 @@
-"""GMFSS Fortuna (union) on B200 - SURVEY.md section 8 row a11 / BASELINE.json configs[3].
+"""GMFSS Fortuna (union) on H100 - SURVEY.md section 8 row a11 / BASELINE.json configs[3].
 
 Host schedule of `vfi_models/gmfss_fortuna/GMFSS_Fortuna_union_arch.py`: `Model.reuse` :1726-1782 (GMFlow in both directions
 on the half-size frames, MetricNet, FeatureNet) and `Model.inference` :1784-1857 (eight soft splats, the RIFE 4.6 sub-model,

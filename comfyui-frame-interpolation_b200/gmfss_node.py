@@ -1,4 +1,4 @@
-"""ComfyUI node surface of the B200 GMFSS Fortuna path: a drop-in for the reference's `GMFSS Fortuna VFI` node
+"""ComfyUI node surface of the H100 GMFSS Fortuna path: a drop-in for the reference's `GMFSS Fortuna VFI` node
 (vfi_models/gmfss_fortuna/__init__.py:79-143): same attributes and kwargs; the model call inside
 `generic_frame_loop(..., use_timestep=True)` is `gmfss.GMFSS.interpolate` (libvfi_b200.so kernels), no fallback.
 Only the `GMFSS_fortuna_union` configuration (the one SURVEY.md section 8 / BASELINE.json configs[3] name) is built."""

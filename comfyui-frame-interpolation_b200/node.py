@@ -1,4 +1,4 @@
-"""ComfyUI node surface of the B200 path: a drop-in for the reference's `RIFE VFI` node.
+"""ComfyUI node surface of the H100 path: a drop-in for the reference's `RIFE VFI` node.
 
 Mirrors vfi_models/rife/__init__.py:34-239 (class attributes, kwargs, task order, skip / multiplier-list
 semantics, output assembly, dtype round trip) and vfi_utils.py:49-81, :391-407 (InterpolationStateList,

@@ -1,5 +1,5 @@
 """Op-level surface of the reference's `vfi_models.ops` package (vfi_models/ops/__init__.py:19-21), backed by the
-ahead-of-time sm_100a kernels in libvfi_b200.so instead of cupy/NVRTC or taichi.  Same names, argument meaning and
+ahead-of-time sm_90a kernels in libvfi_b200.so instead of cupy/NVRTC or taichi.  Same names, argument meaning and
 tensor contract (CUDA float32 NCHW); inference only - the reference's backward kernels (training) are out of scope.
 There is no CPU path: CPU tensors raise.
 """

@@ -1,4 +1,4 @@
-"""ComfyUI node surface of the B200 Sepconv path: a drop-in for the reference's `Sepconv VFI` node
+"""ComfyUI node surface of the H100 Sepconv path: a drop-in for the reference's `Sepconv VFI` node
 (vfi_models/sepconv/__init__.py:13-57): same attributes and kwargs; the model call inside
 `generic_frame_loop(..., use_timestep=False)` is `SepconvEngine.middle_frame` (libvfi_b200.so), no fallback."""
 import typing
@@ -120,7 +120,9 @@ class SepconvVFI:
         **kwargs
     ):
         engine = kwargs.pop("_engine", None) or _load_engine(ckpt_name)
-        if type(multiplier) == int and multiplier == 2 and frames.shape[0] >= 2 and torch.cuda.is_available():
+        # the pipelined path drives the library engine's device buffers; any other middle-frame model (a caller-supplied
+        # engine) goes through the generic loop, whether or not a GPU is present
+        if type(multiplier) == int and multiplier == 2 and frames.shape[0] >= 2 and isinstance(engine, SepconvEngine):
             return (_vfi_x2_pipelined(engine, frames, optional_interpolation_states),)
         x = frames[..., :3].permute(0, 3, 1, 2)   # preprocess_frames, vfi_utils.py:139-140
 

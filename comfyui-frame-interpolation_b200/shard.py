@@ -113,17 +113,15 @@ class PushGather:
 
     dist.gather is NCCL send / recv: its kernels need SMs on both ends, and every hot kernel of this path is a persistent
     grid of exactly one CTA per SM - with a few SMs taken by NCCL the last CTAs of each layer wait for a free SM and the
-    layer takes up to twice as long (r02, N = 2: 21.7 -> 26.7 ms per step with the chunked NCCL gather, the same 26.7 ms as
-    in r01 although the step itself had become 3.4 ms faster).  Here the destination rank allocates one [world, rows, ...]
+    layer can take up to twice as long.  Here the destination rank allocates one [world, rows, ...]
     buffer, shares it through CUDA IPC, and every rank writes its rows straight into its slice with an ordinary
     device-to-device copy on a side stream (a peer copy = DMA engines over NVLink / NVSwitch, no SMs anywhere), chunk by
     chunk behind the kernels that produce them.  torch.distributed (NCCL) carries the IPC handle once and the barrier that
     ends a step.
 
-    Measured r02 (profiles/r02_n2c_probe.log): correct, but 35 GB/s - inside this pool's containers the IPC mapping gets no
-    NVLink peer access and the copy is staged through host memory - against 595 GB/s for the NCCL gather, so bench.py keeps
-    the NCCL gather (in chunks of one internal pass) and this class is opt-in (VFI_GATHER=push) for hosts where IPC peer
-    mappings work."""
+    Where the IPC mapping gets no NVLink peer access (some containers) the copy is staged through host memory and is far
+    slower than the NCCL gather, so bench.py keeps the NCCL gather (in chunks of one internal pass) and this class is
+    opt-in (VFI_GATHER=push) for hosts where IPC peer mappings work."""
 
     def __init__(self, rows: int, row_shape, dtype, dist, dst: int = 0, device=None):
         import torch.multiprocessing.reductions as red

@@ -1,4 +1,4 @@
-/* libvfi_b200.so - C ABI of the B200-native frame-interpolation hot path (RIFE 4.6 first).
+/* libvfi_b200.so - C ABI of the H100-native frame-interpolation hot path (RIFE 4.6 first).
  *
  * The reference (Fannovel16/ComfyUI-Frame-Interpolation @ 26545cc) has no native library: its "FFI" is
  * (a) PyTorch ATen calls from vfi_models/rife/rife_arch.py and (b) cupy RawModule launches that pass
@@ -144,7 +144,7 @@ int vfi_film_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* nume
  * pyramid levels), any other size as in the reference.  Asynchronous on `stream`. */
 int vfi_film_forward(vfi_ctx* ctx, const float* frames, int n_frames, int H, int W, int C, const int32_t* f0,
                      const int32_t* f1, int n_pairs, int clamp01, float* out, void* stream);
-/* Test / profiling hooks: route every FILM conv through the CUDA-core checker (1) or the tcgen05 kernel (0); run one
+/* Test / profiling hooks: route every FILM conv through the CUDA-core checker (1) or the wgmma kernel (0); run one
  * conv layer (group 0 = extract: layer 2*j + {0,1}; 1 = flow estimators: 4*predictor + conv; 2 = fusion: 3*k + conv)
  * on caller tensors (16-bit NHWC channel slices: pointer + pixel pitch in elements); static plan of a layer; tensor-core
  * MACs (unpadded channels) of the last forward. */
@@ -172,7 +172,7 @@ int vfi_sepconv_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* n
  * the reference); f0 / f1: HOST index arrays.  Any H, W >= 2.  Asynchronous on `stream`. */
 int vfi_sepconv_forward(vfi_ctx* ctx, const float* frames, int n_frames, int H, int W, int C, const int32_t* f0,
                         const int32_t* f1, int n_pairs, float* out, void* stream);
-/* Test hooks: every conv through the CUDA-core checker (1) / the tcgen05 kernel (0); the host-only weight packer of
+/* Test hooks: every conv through the CUDA-core checker (1) / the wgmma kernel (0); the host-only weight packer of
  * vfi_sepconv_load (a 3x3 conv packed as a stride-1 layer, or as the 2x2 conv over the space-to-depth input that runs
  * its stride-2 form). */
 int vfi_sepconv_debug_set_ref(vfi_ctx* ctx, int use_ref);
@@ -184,7 +184,7 @@ int vfi_sepconv_debug_pack_host(int stride2, int cin, int cout, int n_total, int
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
  * [B, 4H, 4W, 8] 16-bit.  `in`/`out` are device tensors in the kernel-native layouts documented in DESIGN.md
  * (16-bit NHWC; layers 0/1 read space-to-depth inputs; layer 10 writes float4 flow + float mask planes).
- * impl 0 = tcgen05 kernel, 1 = CUDA-core checker with the same packed weights. */
+ * impl 0 = wgmma kernel, 1 = CUDA-core checker with the same packed weights. */
 int vfi_rife46_debug_layer(vfi_ctx* ctx, int block, int layer, const void* in, void* out, void* out_mask, int B, int H,
                            int W, int impl, void* stream);
 /* Copies the full-resolution flow (float4 [batch,Hp,Wp]) and mask (float [batch,Hp,Wp]) of the LAST internal

@@ -2,7 +2,7 @@
 
 The reference's custom ops are CUDA C strings launched through cupy (``vfi_models/ops/cupy_ops/{softsplat,costvol,
 sepconv}.py``); neither cupy nor a GPU exists in the build container, which left ``oracle/ops_ref.py`` (the CPU
-restatements the GPU tests check the sm_100a op kernels against) pinned only to a reading of those strings.  This module
+restatements the GPU tests check the sm_90a op kernels against) pinned only to a reading of those strings.  This module
 closes that gap without copying any reference source into the repo:
 
   1. the reference modules are imported from ``/root/reference`` as they are (with a stub ``cupy`` module: only
@@ -15,7 +15,7 @@ closes that gap without copying any reference source into the repo:
      (``args = [n, data pointers...]``, one emulated thread walking the whole grid-stride range).
 
 ``tests/test_ops_ref_pinned.py`` holds ``oracle/ops_ref.py`` to these outputs, which makes the chain
-reference kernel source -> oracle -> sm_100a kernels (GPU tests) complete for softsplat_out, costvol_out and sepconv_out.
+reference kernel source -> oracle -> sm_90a kernels (GPU tests) complete for softsplat_out, costvol_out and sepconv_out.
 ``kernel_Correlation_rearrange`` / ``_updateOutput`` (blocks of cooperating threads, shared memory, ``__syncthreads``) run
 through a second shim, ``tests/host_emu/block_emu.h``: every thread of a block is a fiber and ``__syncthreads()`` yields to
 a round-robin scheduler, i.e. the block advances barrier phase by barrier phase in thread order (warp lock-step).

@@ -101,8 +101,8 @@ static inline cudaError_t emu_malloc(void** p, size_t n) {
 }
 static inline cudaError_t emu_props(cudaDeviceProp* p, int) {
   std::memset(p, 0, sizeof(*p));
-  p->major = 10;
-  p->multiProcessorCount = 148;
+  p->major = 9;
+  p->multiProcessorCount = 132;
   return cudaSuccess;
 }
 static inline cudaError_t emu_memcpy(void* d, const void* s, size_t n) {

@@ -1,7 +1,7 @@
 // Whole-path host emulation of the FILM path (TEST INFRASTRUCTURE): csrc/film.cu (weight loading / channel maps, the forward
 // schedule of ~190 launches, buffer sizing, the C ABI), csrc/film_elem.cu and csrc/streamconv.cu's packer + CUDA-core
-// checker kernel, compiled for the host through cuda_shim.h.  The tcgen05 kernel is not emulated (the checker stands in, as
-// `vfi_film_debug_set_ref(ctx, 1)` selects on a GPU; tcgen05 vs checker is a GPU test).
+// checker kernel, compiled for the host through cuda_shim.h.  The wgmma kernel is not emulated (the checker stands in, as
+// `vfi_film_debug_set_ref(ctx, 1)` selects on a GPU; wgmma vs checker is a GPU test).
 #include "cuda_shim.h"
 
 #include <string>
@@ -15,7 +15,7 @@ struct vfi_ctx {
 namespace vfi {
 static std::string g_err;
 void set_error(const std::string& s) { g_err = s; }
-CtxInfo ctx_info(::vfi_ctx*) { return CtxInfo{0, 148, nullptr, nullptr, nullptr}; }
+CtxInfo ctx_info(::vfi_ctx*) { return CtxInfo{0, 132, nullptr, nullptr, nullptr}; }
 FilmState*& ctx_film(::vfi_ctx* c) { return c->film; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi

@@ -1,7 +1,7 @@
 // Whole-path host emulation of the RIFE path (TEST INFRASTRUCTURE): csrc/rife46.cu (context, weight repacking, the forward
 // schedule, the host pipeline, the C ABI), csrc/elementwise.cu (prep / front / final / warp kernels) and csrc/tapconv.cu's
-// plan + CUDA-core checker kernel, compiled for the host through cuda_shim_block.h.  The tcgen05 kernel is not emulated
-// (launch_tapconv falls back to the checker with the same packed weights; tcgen05 vs checker is tests/test_gpu_layers.py).
+// plan + CUDA-core checker kernel, compiled for the host through cuda_shim_block.h.  The wgmma kernel is not emulated
+// (launch_tapconv falls back to the checker with the same packed weights; wgmma vs checker is tests/test_gpu_layers.py).
 #include "cuda_shim_block.h"
 
 #include <string>

@@ -1,7 +1,7 @@
 // Whole-path host emulation of the Sepconv trunk (TEST INFRASTRUCTURE): csrc/sepconv.cu (weight loading, the forward
 // schedule, buffer sizing, the C ABI), csrc/sepconv_elem.cu and csrc/streamconv.cu's packer + CUDA-core checker kernel,
 // and csrc/ops.cu's tiled separable-convolution kernel, compiled for the host through cuda_shim_block.h (blocks on host
-// threads, threads as fibers).  What is NOT emulated: the tcgen05 kernel (the checker stands in, exactly as
+// threads, threads as fibers).  What is NOT emulated: the wgmma kernel (the checker stands in, exactly as
 // `vfi_sepconv_debug_set_ref(ctx, 1)` selects on a GPU).
 #include "cuda_shim_block.h"
 
@@ -16,7 +16,7 @@ struct vfi_ctx {
 namespace vfi {
 static std::string g_err;
 void set_error(const std::string& s) { g_err = s; }
-CtxInfo ctx_info(::vfi_ctx*) { return CtxInfo{0, 148, nullptr, nullptr, nullptr}; }
+CtxInfo ctx_info(::vfi_ctx*) { return CtxInfo{0, 132, nullptr, nullptr, nullptr}; }
 SepState*& ctx_sep(::vfi_ctx* c) { return c->sep; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi

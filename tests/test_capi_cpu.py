@@ -17,7 +17,7 @@ def test_library_exports_every_declared_symbol(pkg):
     L = ctypes.CDLL(_lib.LIB_PATH)
     for s in declared:
         assert hasattr(L, s), s
-    assert b"sm_100a" in _lib.lib().vfi_version()
+    assert b"sm_90a" in _lib.lib().vfi_version()
 
 
 def test_no_gpu_is_a_loud_error(pkg):
@@ -119,7 +119,7 @@ def test_ops_module_has_every_name_the_reference_exports(pkg):
              "batch_edt", "FunctionAdaCoF", "ModuleCorrelation", "FunctionCorrelation", "_FunctionCorrelation"]
     for n in names:
         assert hasattr(ops, n), n
-    ref_init = "/root/reference/vfi_models/ops/__init__.py"
-    if os.path.exists(ref_init):   # build container: the list above IS the reference's
-        line = [ln for ln in open(ref_init) if "from .cupy_ops import" in ln][0]
-        assert sorted(x.strip() for x in line.split("import", 1)[1].split(",")) == sorted(names)
+    # the reference's import line (vfi_models/ops/__init__.py:21), stored verbatim
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_ops_exports.txt")) as f:
+        line = f.read()
+    assert sorted(x.strip() for x in line.split("import", 1)[1].split(",")) == sorted(names)

@@ -1,7 +1,7 @@
 """The WHOLE FILM path of the library on the CPU: csrc/film.cu (vfi_film_load + vfi_film_forward: 82 tensors, channel maps,
 buffer sizing, the ~190-launch schedule), csrc/film_elem.cu and streamconv.cu's packer + CUDA-core checker kernel, compiled
 for the host (tests/host_emu, one host thread per emulated block) and compared with the output of the unmodified reference
-Interpolator (tests/golden/film_net_64x64_rand.npz, white-noise frames outside [0, 1]).  The tcgen05 kernel is not part of
+Interpolator (tests/golden/film_net_64x64_rand.npz, white-noise frames outside [0, 1]).  The tensor-core kernel is not part of
 this; tools/film_gpu_check.py compares it with the same checker kernel on the GPU."""
 import ctypes as C
 import math

@@ -1,7 +1,7 @@
 """FILM node host logic on CPU: schedule, skip / multiplier-list semantics and output assembly of
 comfyui-frame-interpolation_b200/film_node.py against the outputs of the unmodified reference node
 (tests/golden/film_node_*.npz).  The model call is a stand-in here (the CPU oracle behind the engine's
-``forward`` signature) - the product engine needs a B200 and is covered by the GPU tests."""
+``forward`` signature) - the product engine needs an H100 and is covered by the GPU tests."""
 import os
 import sys
 

@@ -1,7 +1,7 @@
 """-m gpu: parity AT THE CONFIGURATIONS THE NUMBERS ARE QUOTED ON (BASELINE.json configs[0] and configs[1]).
 
 * config 1: the reference's demo pair (540 x 960) through the node mirror vs the unmodified reference node's output.
-* config 2 geometry: 1080 x 1920 (padded 1088 x 1920), a pass of B = 8 pairs (the bench's internal batch: 148 persistent
+* config 2 geometry: 1080 x 1920 (padded 1088 x 1920), a pass of B = 8 pairs (the bench's internal batch: 132 persistent
   CTAs striding > 8 k tiles per layer) vs (a) the unmodified reference's crops / box-filtered frame and (b) the oracle's
   full frames computed on this box's CPU.
 Tolerance (north_star): PSNR >= 50 dB on the interpolated frames; pass-through frames bit exact."""

@@ -51,8 +51,8 @@ def test_warp_primitive(engines):
         assert (out - ref).abs().max().item() < 3e-5  # the reference's normalise/denormalise rounding
 
 
-IMPLS = [pytest.param(1, id="ref"), pytest.param(0, id="tc")]  # CUDA-core checker / tcgen05 kernel
-# (impl, dtype) pairs: the tcgen05 kernel in both operand types, the CUDA-core checker in one (no skipped combinations)
+IMPLS = [pytest.param(1, id="ref"), pytest.param(0, id="tc")]  # CUDA-core checker / wgmma kernel
+# (impl, dtype) pairs: the wgmma kernel in both operand types, the CUDA-core checker in one (no skipped combinations)
 IMPL_DTYPE = [pytest.param(1, "float16", id="ref-float16"), pytest.param(0, "float16", id="tc-float16"),
               pytest.param(0, "bfloat16", id="tc-bfloat16")]
 
@@ -74,8 +74,8 @@ def test_resconv(engines, block, dtype, impl):
 
 @pytest.mark.parametrize("block", [3, 1, 0])
 def test_resconv_many_tiles(engines, block):
-    """More tiles than persistent CTAs: every CTA walks several tiles, so the window stages / ring slots, both TMEM
-    accumulators and all mbarrier phases wrap several times (blocks 0 and 1 run the k-block ring pipeline)."""
+    """More tiles than persistent CTAs: every CTA walks several tiles, so the window stages / ring slots, both MMA warpgroups'
+    tiles and all mbarrier phases wrap several times (blocks 0 and 1 run the k-block ring pipeline)."""
     sd, e = engines
     eng, c = e["float16"], BLOCK_C[block]
     g = torch.Generator().manual_seed(40 + block)

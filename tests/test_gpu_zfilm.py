@@ -1,9 +1,8 @@
 """FILM on the GPU (SURVEY.md section 8 row a10): tools/film_gpu_check.py --quick in a SUBPROCESS (a kernel trap in
 the newest kernels must not poison the CUDA context of the RIFE tests that share this pytest process; the file name
-sorts it after them).  The checker reports, stage by stage: single streamconv layers (tcgen05 kernel vs the CUDA-core
-checker vs torch conv2d with the layer's real weights), the whole network on the checker and on the tcgen05 kernel vs
-the unmodified reference's output (PSNR >= 50 dB), and the node vs the unmodified reference node.  First GPU run:
-profiles/r01_film_gpu_check.jsonl (14 / 14 stages, 64.4 dB net, 83.7 dB node)."""
+sorts it after them).  The checker reports, stage by stage: single streamconv layers (wgmma kernel vs the CUDA-core
+checker vs torch conv2d with the layer's real weights), the whole network on the checker and on the wgmma kernel vs
+the unmodified reference's output (PSNR >= 50 dB), and the node vs the unmodified reference node."""
 import os
 import subprocess
 import sys

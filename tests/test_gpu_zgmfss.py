@@ -1,4 +1,4 @@
-"""-m gpu: GMFSS Fortuna (union) on the B200 (SURVEY.md section 8 row a11): gmops kernels + fused soft splat + RIFE engine under
+"""-m gpu: GMFSS Fortuna (union) on the H100 (SURVEY.md section 8 row a11): gmops kernels + fused soft splat + RIFE engine under
 the product's schedule against outputs of the UNMODIFIED reference model (tests/golden/gmfss_*.npz), and the node mirror.
 The same schedule is pinned on the CPU through a host build of the kernels (tests/test_gmfss_host.py)."""
 import os

@@ -1,5 +1,4 @@
-"""FunctionAdaCoF / batch_edt on the GPU vs the oracle (pinned to the reference's kernels on the CPU).  The kernels were
-written after r01's last GPU minute; first GPU run r02 (profiles/r02_a_gpu_tests.log): green."""
+"""FunctionAdaCoF / batch_edt on the GPU vs the oracle (pinned to the reference's kernels on the CPU)."""
 import pytest
 import torch
 

@@ -1,6 +1,5 @@
 """RIFE node scale_factor 2 / 4 (up-scaled last blocks, archs 4.6 / 4.7 / 4.17 / 4.26) on the GPU against the unmodified reference's outputs.
-front_up / fold_down were written after r01's last GPU minute and verified through the host emulation only
-(tests/test_rife_full_host.py: 97 - 105 dB); first GPU run r02: green (profiles/r02_a_gpu_tests.log)."""
+front_up / fold_down are also checked through the host emulation (tests/test_rife_full_host.py)."""
 import os
 import sys
 

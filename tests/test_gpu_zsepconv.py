@@ -1,7 +1,6 @@
 """Sepconv on the GPU (SURVEY.md section 8 row a12): tools/sepconv_gpu_check.py in a SUBPROCESS (sorted after the verified
-tests; a trap in new code must not poison their CUDA context).  The Sepconv trunk was written at the end of r01 with no
-GPU minutes left; its first GPU run (r02, profiles/r02_sepconv_gpu_check.jsonl) was green on every stage: 98 - 101 dB on
-the tcgen05 kernel vs the unmodified reference Network."""
+tests; a trap in new code must not poison their CUDA context): every stage, on the CUDA-core checker and on the wgmma
+kernel, vs the unmodified reference Network."""
 import os
 import subprocess
 import sys

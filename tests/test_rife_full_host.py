@@ -2,7 +2,7 @@
 repacking, the per-block schedule with its implicit full-resolution flow, the C ABI), csrc/elementwise.cu (prep / front /
 final kernels with their 3-D launch geometry) and csrc/tapconv.cu's plan + CUDA-core checker kernel, compiled for the host
 (tests/host_emu/cuda_shim_block.h: every thread of every block a fiber) and compared with the unmodified reference IFNet's
-output (tests/golden).  The tcgen05 kernel is covered by the GPU tests (tests/test_gpu_layers.py: tcgen05 vs this checker)."""
+output (tests/golden).  The wgmma kernel is covered by the GPU tests (tests/test_gpu_layers.py: wgmma vs this checker)."""
 import ctypes as C
 import math
 import os

@@ -2,7 +2,7 @@
 PReLU slopes, buffer sizing, the schedule with its crop-after-conv decoder path), csrc/sepconv_elem.cu and streamconv.cu's
 packer + CUDA-core checker kernel, compiled for the host (tests/host_emu) and compared with the output of the unmodified
 reference Network (tests/golden/sepconv_net_*.npz, three sizes).  ops.cu's tiled
-separable-convolution kernel runs too; only the tcgen05 kernel is replaced (by the checker kernel with the same weights)."""
+separable-convolution kernel runs too; only the tensor-core kernel is replaced (by the checker kernel with the same weights)."""
 import ctypes as C
 import math
 import os

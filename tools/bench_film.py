@@ -150,7 +150,7 @@ def main():
                       "interpolated frames/sec @%dx%d FILM %dx" % (W, H, m),
             "value": value, "unit": "frames/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
             "ms_per_step": ms_dev / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f16", "dtype_note": "conv operands fp16, fp32 accumulate (TMEM); images, flows, warps' weights fp32",
+            "dtype": "f16", "dtype_note": "conv operands fp16, fp32 accumulate (registers); images, flows, warps' weights fp32",
             "data": "synthetic",
             "config": {"workload": f"FILM VFI, {m}x multiplier, {nf}-frame synthetic {H}x{W} clip per GPU "
                                    f"(BASELINE configs[2] shape; {nf - 1} pairs x {m - 1} forward calls)",

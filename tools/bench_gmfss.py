@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GMFSS Fortuna harness (BASELINE.json configs[3]: GMFSS Fortuna union, 2x, 720p on 1 x B200; `bench.py` metric family).
+"""GMFSS Fortuna harness (BASELINE.json configs[3]: GMFSS Fortuna union, 2x, 720p on 1 x H100; `bench.py` metric family).
 
     python tools/bench_gmfss.py [--h 720 --w 1280] [--steps 3] [--warmup 2]
 
@@ -18,7 +18,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-FP32_FMA_TFLOPS = 74.5  # 148 SMs x 128 lanes x 2 x 1.965 GHz
+FP32_FMA_TFLOPS = 67.0  # H100 SXM data sheet, FP32
 
 
 def main():
@@ -93,7 +93,7 @@ def main():
             "ms_reuse": ms_reuse / a.steps, "ms_inference": ms_inf / a.steps, "finite": bool(torch.isfinite(out).all()),
             "roofline": {"bound": "fp32 FMA", "kernel": "whole frame (gmops conv / gemm + element-wise + splats + RIFE)", "achieved": tf,
                          "peak": FP32_FMA_TFLOPS, "unit": "TFLOP/s", "frac": tf / FP32_FMA_TFLOPS, "gmacs_per_frame": macs["n"] / 1e9,
-                         "peak_source": "nominal: 148 SMs x 128 lanes x 2 x 1.965 GHz", "traffic": None}}
+                         "peak_source": "H100 SXM data sheet (FP32)", "traffic": None}}
     if not a.no_cpu:
         torch.set_num_threads(min(32, os.cpu_count() or 1))
         hs, ws = 192, 256

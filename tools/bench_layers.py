@@ -23,7 +23,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--json", default="")
     ap.add_argument("--only", default="", help="block:layer, e.g. 3:2")
-    ap.add_argument("--lib", default="", help="alternate libvfi_b200 build (diagnostic builds, tools/ablate.sh)")
+    ap.add_argument("--lib", default="", help="alternate libvfi_b200 build (diagnostic builds)")
     a = ap.parse_args()
     ge.load_package()
     if a.lib:

@@ -49,7 +49,7 @@ def main():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         peaks = json.load(open(p))
-    fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e9  # GFLOP/s, CUDA-core FMA peak at the maximum SM clock
+    fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e9  # GFLOP/s, H100 SXM CUDA-core FMA peak at the maximum SM clock
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     rows = []
 

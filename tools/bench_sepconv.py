@@ -28,7 +28,7 @@ sys.path.insert(0, ROOT)
 
 TRUNK_MACS_PER_PX = 479e3   # conv trunk incl. the four 51-channel heads (SURVEY.md section 8 a12, probe)
 OP_MACS_PER_PX = 20.8e3     # adaptive separable convolution: 2 frames x 51 x 51 taps x 4 channels (fp32 CUDA cores)
-FP32_FMA_TFLOPS = 74.5      # 148 SMs x 128 FMA lanes x 2 flop x 1.965 GHz (no measured figure in MEASURED_PEAKS.json)
+FP32_FMA_TFLOPS = 67.0      # H100 SXM data sheet, FP32 (no measured figure in MEASURED_PEAKS.json)
 
 
 def main():
@@ -131,7 +131,7 @@ def main():
         line = {"metric": f"interpolated frames/sec @{W}x{H} Sepconv 2x", "value": value, "unit": "frames/s", "n_gpus": world,
                 "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_dev / a.steps, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "f16",
-                "dtype_note": "trunk conv operands fp16, fp32 accumulate (TMEM); the separable-convolution op fp32", "data": "synthetic",
+                "dtype_note": "trunk conv operands fp16, fp32 accumulate (registers); the separable-convolution op fp32", "data": "synthetic",
                 "config": {"workload": f"Sepconv VFI, 2x multiplier, {nf}-frame synthetic {H}x{W} clip per GPU (BASELINE configs[4] shape)",
                            "pairs_per_call": a.pairs,
                            "parallelism": f"frame-pair shards x{world}, output frames gathered on rank 0 by NCCL" if world > 1 else "1 GPU",
@@ -163,7 +163,7 @@ def main():
         op_tf = 2.0 * (OP_MACS_PER_PX / 2) * he * we / (op_ms * 1e-3) / 1e12
         line["roofline_op"] = {"bound": "fp32 FMA", "kernel": "sepconv_tile_kernel (K = 51, RGB + ones, one frame)", "launch_ms": op_ms,
                                "achieved": op_tf, "peak": FP32_FMA_TFLOPS, "unit": "TFLOP/s", "frac": op_tf / FP32_FMA_TFLOPS,
-                               "peak_source": "nominal: 148 SMs x 128 lanes x 2 x 1.965 GHz"}
+                               "peak_source": "H100 SXM data sheet (FP32)"}
         if world == 1 and not a.no_cpu:
             torch.set_num_threads(min(32, os.cpu_count() or 1))
             hs, ws = 270, 480

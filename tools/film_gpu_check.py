@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""FILM on the GPU, checked stage by stage (run on a B200 box; tests/test_gpu_zfilm.py runs it in a subprocess).
+"""FILM on the GPU, checked stage by stage (run on an H100; tests/test_gpu_zfilm.py runs it in a subprocess).
 
     python tools/film_gpu_check.py [--quick]
 
 Stages, each reported as one JSON line {"stage": ..., "ok": ..., ...}; exit code 0 only if every stage passed:
-  conv:<group>.<layer>   one streamconv layer on random 16-bit inputs: tcgen05 kernel vs the CUDA-core checker (same
+  conv:<group>.<layer>   one streamconv layer on random 16-bit inputs: wgmma kernel vs the CUDA-core checker (same
                          packed weights) and, for layers whose input channels are in reference order, vs torch conv2d
                          on the CPU with the layer's real weights
   forward_ref / forward  Interpolator.forward through libvfi_b200.so with every conv on the CUDA-core checker / on the
-                         tcgen05 kernel, vs the unmodified reference's output (tests/golden/film_net_*.npz): PSNR >= 50 dB
+                         wgmma kernel, vs the unmodified reference's output (tests/golden/film_net_*.npz): PSNR >= 50 dB
                          and the five flow-pyramid levels within 0.05 px RMS
   node                   FILM_VFI.vfi vs the unmodified reference node's output (tests/golden/film_node_*.npz)
 The oracle / goldens are the checker here, never the thing measured.
@@ -146,9 +146,9 @@ def main():
 
     bad = [r["stage"] for r in RESULTS if not r["ok"]]
     print(json.dumps(dict(summary=True, stages=len(RESULTS), failed=bad)), flush=True)
-    out_dir = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(out_dir):
-        with open(os.path.join(out_dir, "film_gpu_check.jsonl"), "w") as fh:
+    out_path = os.environ.get("VFI_CHECK_JSONL")  # optional: every stage's record as one JSON line each
+    if out_path:
+        with open(out_path, "w") as fh:
             for r in RESULTS:
                 fh.write(json.dumps(r) + "\n")
     return 1 if bad else 0

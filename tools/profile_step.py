@@ -3,7 +3,7 @@
 lists and `--set full` captures (bench.py itself also runs the node, the CPU leg and the stand-alone kernel timings).
 
     ncu --metrics gpu__time_duration.sum --clock-control none -s <launches of the warm-up pass> -c 60 --csv \
-        --log-file gpurun_out/launches.csv python tools/profile_step.py --frames 9 --iters 2
+        --log-file launches.csv python tools/profile_step.py --frames 9 --iters 2
 """
 import argparse
 import os

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Sepconv on the GPU, checked against the unmodified reference's outputs (run on a B200 box;
+"""Sepconv on the GPU, checked against the unmodified reference's outputs (run on an H100;
 tests/test_gpu_zsepconv.py runs it in a subprocess).
 
     python tools/sepconv_gpu_check.py
 
 One JSON line per stage; exit code 0 only if every stage passed:
   forward_ref:<case> / forward:<case>   Network.forward through libvfi_b200.so with every conv on the CUDA-core checker /
-                                        on the tcgen05 kernel vs tests/golden/sepconv_net_*.npz (PSNR >= 50 dB); the
+                                        on the wgmma kernel vs tests/golden/sepconv_net_*.npz (PSNR >= 50 dB); the
                                         45x54 case has odd rows down the pyramid (crop-after-conv path of the decoder)
   batch                                 two pairs in one call == the two single calls
   node                                  SepconvVFI.vfi (multiplier 3) == the bisection of single engine calls
@@ -92,9 +92,9 @@ def main():
 
     bad = [r["stage"] for r in RESULTS if not r["ok"]]
     print(json.dumps(dict(summary=True, stages=len(RESULTS), failed=bad)), flush=True)
-    out_dir = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(out_dir):
-        with open(os.path.join(out_dir, "sepconv_gpu_check.jsonl"), "w") as fh:
+    out_path = os.environ.get("VFI_CHECK_JSONL")  # optional: every stage's record as one JSON line each
+    if out_path:
+        with open(out_path, "w") as fh:
             for r in RESULTS:
                 fh.write(json.dumps(r) + "\n")
     return 1 if bad else 0
