@@ -20,5 +20,5 @@ NODE_DISPLAY_NAME_MAPPINGS = {
     "RIFE VFI": "RIFE VFI (H100 native, rife4.6)",
     "FILM VFI": "FILM VFI (H100 native)",
     "Sepconv VFI": "Sepconv VFI (H100 native)",
-    "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native, union)",
+    "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native)",
 }

@@ -1,4 +1,4 @@
-"""GMFSS Fortuna (union) on H100 - SURVEY.md section 8 row a11 / BASELINE.json configs[3].
+"""GMFSS Fortuna on H100 - SURVEY.md section 8 row a11 / BASELINE.json configs[3].
 
 Host schedule of `vfi_models/gmfss_fortuna/GMFSS_Fortuna_union_arch.py`: `Model.reuse` :1726-1782 (GMFlow in both directions
 on the half-size frames, MetricNet, FeatureNet) and `Model.inference` :1784-1857 (eight soft splats, the RIFE 4.6 sub-model,
@@ -8,6 +8,10 @@ operation is a kernel of libvfi_b200.so: the fp32 building blocks of csrc/gmops.
 There is no PyTorch / CPU fallback on the product path.  (tests/ run this same schedule on CPU tensors against a host build
 of gmops.cu - `Ops(lib=<emulation library>)` - with the oracle standing in for the two components that have their own GPU
 tests, the splat and the RIFE engine.)
+
+The same class serves the base model, `GMFSS_Fortuna_arch.py` (the `GMFSS_fortuna` checkpoint), chosen by the weights: a set
+without `ifnet` is the base model.  It has no RIFE sub-model, and GridNet's first head (`residual_model_head`, 12 input
+channels) reads `[h0, splat(h0), splat(h1), h1]` instead of `[splat(h0), rife, splat(h1)]` (base :1843-1848).
 
 Tensors are NCHW float32 like the reference's; weights are the reference's state_dicts, used in place.
 """
@@ -300,9 +304,14 @@ def _shift_mask(h: int, w: int, splits: int) -> torch.Tensor:
 
 class GMFSS:
     """`sds`: {"flownet", "metricnet", "feat_ext", "fusionnet", "ifnet"} state_dicts of the reference's five sub-networks
-    (gmfss_fortuna/__init__.py:27-39 loads them from five checkpoint files)."""
+    (gmfss_fortuna/__init__.py:27-39 loads them from five checkpoint files) for the union model, the same without "ifnet"
+    (four files) for the base model; `self.variant` ("union" / "base") records which.  The base model takes no `rife`."""
 
     def __init__(self, sds: Dict[str, Dict[str, torch.Tensor]], ops: Ops, splat=None, rife=None):
+        self.variant = "union" if "ifnet" in sds else "base"
+        self._head = "head0" if self.variant == "union" else "head"
+        if f"residual_model_{self._head}.1.weight" not in sds["fusionnet"]:
+            raise KeyError(f"GMFSS {self.variant}: fusionnet has no residual_model_{self._head} (GridNet of the other variant?)")
         self.o = ops
         dev = ops.dev
         self.sd = {net: {k: v.detach().to(dev, torch.float32).contiguous() for k, v in sd.items()} for net, sd in sds.items() if net != "ifnet"}
@@ -317,7 +326,7 @@ class GMFSS:
         self.mean = torch.tensor([0.485, 0.456, 0.406], device=dev)
         self.std = torch.tensor([0.229, 0.224, 0.225], device=dev)
         self.splat = splat     # (x, flow, metric) -> soft splat, NCHW fp32
-        self.rife = rife       # (half0, half1 NCHW fp32, t) -> merged frame NCHW fp32
+        self.rife = rife       # (half0, half1 NCHW fp32, t) -> merged frame NCHW fp32; union only
 
     # ------------------------------------------------------------------ GMFlow (:35-1372)
     def _resblock(self, p, x, stride):
@@ -487,7 +496,7 @@ class GMFSS:
         r = lambda n, t, a=None, b=None: self._block("residual_model_" + n, t, "res", a, b)        # noqa: E731
         d = lambda n, t, a=None, b=None: self._block("downsample_model_" + n, t, "down", a, b)     # noqa: E731
         u = lambda n, t, a=None, b=None: self._block("upsample_model_" + n, t, "up", a, b)         # noqa: E731
-        X00 = r("head1", x1, r("head0", x))
+        X00 = r("head1", x1, r(self._head, x))
         X01 = r("01", X00, X00)
         X10 = d("10", X00, r("head2", x2))
         X20 = d("20", X10, r("head3", x3))
@@ -524,10 +533,17 @@ class GMFSS:
         F1t, F2t = o.axpby(f01, alpha=t), o.axpby(f10, alpha=1.0 - t)
         Z1t, Z2t = o.axpby(m0, alpha=t), o.axpby(m1, alpha=1.0 - t)
         b, _, hh, wh = h0.shape
-        x = o.new(b, 9, hh, wh)
-        o.copy_slice(self.splat(h0, F1t, Z1t), x, 3, 0, 0)
-        o.copy_slice(self.rife(h0, h1, t), x, 3, 0, 3)
-        o.copy_slice(self.splat(h1, F2t, Z2t), x, 3, 0, 6)
+        if self.variant == "union":   # [I1t, rife, I2t]
+            x = o.new(b, 9, hh, wh)
+            o.copy_slice(self.splat(h0, F1t, Z1t), x, 3, 0, 0)
+            o.copy_slice(self.rife(h0, h1, t), x, 3, 0, 3)
+            o.copy_slice(self.splat(h1, F2t, Z2t), x, 3, 0, 6)
+        else:                         # base: [img0, I1t, I2t, img1] of the half-size frames
+            x = o.new(b, 12, hh, wh)
+            o.copy_slice(h0, x, 3, 0, 0)
+            o.copy_slice(self.splat(h0, F1t, Z1t), x, 3, 0, 3)
+            o.copy_slice(self.splat(h1, F2t, Z2t), x, 3, 0, 6)
+            o.copy_slice(h1, x, 3, 0, 9)
         levels = []
         fl1, fl2, z1, z2 = F1t, F2t, Z1t, Z2t
         for lv in range(3):
@@ -559,16 +575,22 @@ class GMFSS:
 
 
 def build_gpu_model(sds: Dict[str, Dict[str, torch.Tensor]], device: int = 0) -> GMFSS:
-    """The product configuration: gmops + fused soft splat + RIFE engine of libvfi_b200.so on cuda:`device`."""
+    """The product configuration: gmops + fused soft splat + RIFE engine of libvfi_b200.so on cuda:`device`.  Without
+    sds["ifnet"] this is the base model: no RIFE engine (and none of its workspace), `_engine` is None."""
     from . import ops as OPS
     from ._lib import lib
-    from .engine import Rife46Engine
     dev = torch.device("cuda", device)
     o = Ops(lib(), dev)
-    eng = Rife46Engine(sds["ifnet"], device=device, dtype="float32", batch=1, arch="4.6")
 
     def splat(x, flow, metric):
         return OPS.softsplat(x, flow, metric, "soft")
+
+    if "ifnet" not in sds:
+        m = GMFSS(sds, o, splat=splat)
+        m._engine = None
+        return m
+    from .engine import Rife46Engine
+    eng = Rife46Engine(sds["ifnet"], device=device, dtype="float32", batch=1, arch="4.6")
 
     def rife(h0, h1, t):
         b, _, h, w = h0.shape

@@ -1,7 +1,9 @@
 """ComfyUI node surface of the H100 GMFSS Fortuna path: a drop-in for the reference's `GMFSS Fortuna VFI` node
 (vfi_models/gmfss_fortuna/__init__.py:79-143): same attributes and kwargs; the model call inside
 `generic_frame_loop(..., use_timestep=True)` is `gmfss.GMFSS.interpolate` (libvfi_b200.so kernels), no fallback.
-Only the `GMFSS_fortuna_union` configuration (the one SURVEY.md section 8 / BASELINE.json configs[3] name) is built."""
+Both checkpoints of the reference's dropdown are served: `GMFSS_fortuna_union` (five files, with the RIFE 4.6 sub-model; the
+configuration SURVEY.md section 8 / BASELINE.json configs[3] name) and `GMFSS_fortuna` (four files, the base model without
+it); `gmfss.build_gpu_model` tells them apart by the presence of `ifnet`."""
 import typing
 
 import torch
@@ -10,7 +12,7 @@ from .frame_loop import generic_frame_loop
 from .node import InterpolationStateList, load_file_from_github_release
 
 GLOBAL_MODEL_TYPE = "gmfss_fortuna"
-# gmfss_fortuna/__init__.py:11-25 (the non-union variant is a different architecture file and is not built)
+# gmfss_fortuna/__init__.py:11-25
 CKPTS_PATH_CONFIG = {
     "GMFSS_fortuna_union": {
         "ifnet": ("rife", "rife46.pth"),
@@ -18,6 +20,12 @@ CKPTS_PATH_CONFIG = {
         "metricnet": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_union_metric.pkl"),
         "feat_ext": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_union_feat.pkl"),
         "fusionnet": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_union_fusionnet.pkl"),
+    },
+    "GMFSS_fortuna": {
+        "flownet": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_flownet.pkl"),
+        "metricnet": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_metric.pkl"),
+        "feat_ext": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_feat.pkl"),
+        "fusionnet": (GLOBAL_MODEL_TYPE, "GMFSS_fortuna_fusionnet.pkl"),
     },
 }
 _model_cache: typing.Dict[str, typing.Any] = {}

@@ -1,16 +1,19 @@
 #!/usr/bin/env python
 """GMFSS Fortuna harness (BASELINE.json configs[3]: GMFSS Fortuna union, 2x, 720p on 1 x H100; `bench.py` metric family).
 
-    python tools/bench_gmfss.py [--h 720 --w 1280] [--steps 3] [--warmup 2]
+    python tools/bench_gmfss.py [--ckpt GMFSS_fortuna_union | GMFSS_fortuna] [--h 720 --w 1280] [--steps 3] [--warmup 2]
 
 One step = one interpolated frame of a device-resident 720p pair through gmfss.GMFSS.interpolate (pad to 768 x 1280, GMFlow in
-both directions, MetricNet, FeatureNet x 2, eight soft splats, RIFE 4.6, GridNet, crop).  Prints ONE JSON line: frames/s,
-the split reuse / inference, fp32 MACs per frame counted from the calls, achieved TFLOP/s against the fp32 FMA rate, and the
-CPU oracle (oracle/gmfss.py == the reference's PyTorch-CPU path) on a small pair scaled by pixel count.
+both directions, MetricNet, FeatureNet x 2, eight soft splats, RIFE 4.6 (union only), GridNet, crop).  `--ckpt` picks the
+node's checkpoint: `GMFSS_fortuna_union` (default) or the base model `GMFSS_fortuna` (no RIFE, 12-channel GridNet input).
+Prints ONE JSON line: frames/s, the split reuse / inference, fp32 MACs per frame counted from the calls, achieved TFLOP/s
+against the fp32 FMA rate, the card's name and power limit, and the CPU oracle (oracle/gmfss.py for union, oracle/gmfss_base.py for base == the
+reference's PyTorch-CPU path) on a small pair scaled by pixel count.
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -19,10 +22,25 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 FP32_FMA_TFLOPS = 67.0  # H100 SXM data sheet, FP32
+VARIANT = {"GMFSS_fortuna_union": "union", "GMFSS_fortuna": "base"}
+
+
+def card(index: int) -> dict:
+    """name and power limit of the card the numbers come from (read only: nvidia-smi --query-gpu)"""
+    import torch
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return info
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--ckpt", choices=list(VARIANT), default="GMFSS_fortuna_union")
     ap.add_argument("--h", type=int, default=720)
     ap.add_argument("--w", type=int, default=1280)
     ap.add_argument("--steps", type=int, default=3)
@@ -34,8 +52,11 @@ def main():
     from cfi_b200.gmfss import build_gpu_model
     from oracle import film as OF
     from oracle import gmfss as OG
+    from oracle import gmfss_base as GB
     from oracle import gmfss_weights as GW
-    sds = GW.synthetic_state_dicts(0)
+    variant = VARIANT[a.ckpt]
+    W, O = (GW, OG) if variant == "union" else (GB, GB)   # seeded weights, CPU oracle
+    sds = W.synthetic_state_dicts(0)
     m = build_gpu_model(sds, 0)
     # count the multiply-accumulates of the conv / gemm calls of one frame
     macs = {"n": 0}
@@ -85,13 +106,17 @@ def main():
         ms_inf += e[1].elapsed_time(e[2])
     ms = (ms_reuse + ms_inf) / a.steps
     tf = 2.0 * macs["n"] / (ms * 1e-3) / 1e12
-    line = {"metric": f"interpolated frames/sec @{a.w}x{a.h} GMFSS Fortuna (union) 2x", "value": 1e3 / ms, "unit": "frames/s", "n_gpus": 1,
+    line = {"metric": f"interpolated frames/sec @{a.w}x{a.h} GMFSS Fortuna ({variant}) 2x", "value": 1e3 / ms, "unit": "frames/s", "n_gpus": 1,
             "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32", "dtype_note": "gmops fp32 on CUDA cores; the RIFE 4.6 sub-model fp16 operands / fp32 accumulate", "data": "synthetic",
-            "config": {"workload": f"GMFSS Fortuna union, 2x, one {a.h}x{a.w} pair per step, device resident (BASELINE configs[3])",
-                       "padded": [ph, pw], "weights": "seeded synthetic (oracle.gmfss_weights.synthetic_state_dicts(0)); no checkpoint ships"},
+            "dtype": "f32", "dtype_note": "gmops fp32 on CUDA cores" + ("; the RIFE 4.6 sub-model fp16 operands / fp32 accumulate"
+                                                                         if variant == "union" else "; no RIFE sub-model"),
+            "data": "synthetic", "gpu": card(0),
+            "config": {"workload": f"GMFSS Fortuna {variant} ({a.ckpt}), 2x, one {a.h}x{a.w} pair per step, device resident"
+                                   + (" (BASELINE configs[3])" if variant == "union" else ""),
+                       "padded": [ph, pw],
+                       "weights": f"seeded synthetic ({W.__name__}.synthetic_state_dicts(0)); no checkpoint ships"},
             "ms_reuse": ms_reuse / a.steps, "ms_inference": ms_inf / a.steps, "finite": bool(torch.isfinite(out).all()),
-            "roofline": {"bound": "fp32 FMA", "kernel": "whole frame (gmops conv / gemm + element-wise + splats + RIFE)", "achieved": tf,
+            "roofline": {"bound": "fp32 FMA", "kernel": "whole frame (gmops conv / gemm + element-wise + splats" + (" + RIFE)" if variant == "union" else ")"), "achieved": tf,
                          "peak": FP32_FMA_TFLOPS, "unit": "TFLOP/s", "frac": tf / FP32_FMA_TFLOPS, "gmacs_per_frame": macs["n"] / 1e9,
                          "peak_source": "H100 SXM data sheet (FP32)", "traffic": None}}
     if not a.no_cpu:
@@ -100,13 +125,14 @@ def main():
         small = OF.synthetic_clip(2, hs, ws, seed=7).permute(0, 3, 1, 2).contiguous()
         t0 = time.perf_counter()
         with torch.no_grad():
-            OG.interpolate(sds, small[0:1], small[1:2], 0.5)
+            O.interpolate(sds, small[0:1], small[1:2], 0.5)
         sec = time.perf_counter() - t0
         line["cpu_baseline"] = {"value": 1.0 / (sec * (ph * pw) / (hs * ws)), "unit": "frames/s", "cores": torch.get_num_threads(), "kind": "port",
-                                "sample": f"one {hs}x{ws} pair ({sec:.1f} s) scaled by pixel count to the padded {ph}x{pw}; oracle/gmfss.py == "
+                                "sample": f"one {hs}x{ws} pair ({sec:.1f} s) scaled by pixel count to the padded {ph}x{pw}; {O.__file__[len(ROOT) + 1:]} == "
                                           "the reference's PyTorch-CPU path with its splat restated on the CPU"}
     print(json.dumps(line))
-    m._engine.close()
+    if m._engine is not None:
+        m._engine.close()
 
 
 if __name__ == "__main__":
