@@ -19,8 +19,11 @@
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles):
 //   warpgroups 0, 1 : MMA + epilogue.  Warpgroup w takes the CTA's tiles w, w + 2, ... and keeps the whole tile's
 //                     accumulators (2 x 64 rows x n_cta columns, fp32) in registers, so one warpgroup's epilogue
-//                     (+shift (+residual) -> LeakyReLU -> 16-bit -> global stores; lastconv: the fp32 4x4 flow/mask
-//                     sub-pixel patch) overlaps the other's MMAs.
+//                     overlaps the other's MMAs: +shift (held in registers for the launch), +residual (non-ring
+//                     ResConv: ldmatrix from the tile's still-held window stage, then the stage is released; ring
+//                     layers: from global memory), LeakyReLU, 16-bit; NHWC outputs are stmatrix'ed into a swizzled
+//                     per-warpgroup staging tile and leave as TMA tensor stores (one thread, clipped at the image
+//                     border); lastconv writes whole float4 flow texels, the space-to-depth forms direct stores.
 //   warp 8          : one elected lane: weight bulk copy, then one 4-D TMA tensor copy per k-block and tile
 #include <cstdlib>
 #include <type_traits>
@@ -54,7 +57,18 @@ __device__ __forceinline__ size_t out_pixel_offset(const TapConvParams& p, int b
   return (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.n_total;
 }
 
+// Channels per TMA store box of a 16-bit NHWC output: the widest of 64 / 32 / 16 that divides the CTA's n_cta, so the
+// box row is 128 / 64 / 32 bytes and uses the swizzle of that width (conflict-free stmatrix into the staging tile).
+__host__ __device__ constexpr int store_box_c(int n_cta) { return n_cta % 64 == 0 ? 64 : n_cta % 32 == 0 ? 32 : 16; }
+
 #ifndef VFI_HOST_EMU  // (tests/host_emu runs the RIFE schedule on the CPU with the checker kernel; no wgmma there)
+// Byte offset of 16-byte chunk `chunk` of row `row` in a 1024-aligned region of rowb-byte rows (32, 64 or 128) laid out
+// by TMA with the swizzle of that width: address bits [4, 4 + log2(rowb / 16)) are XORed with bits [7, ...).
+__device__ __forceinline__ uint32_t swz_off(uint32_t row, uint32_t chunk, uint32_t rowb) {
+  const uint32_t o = row * rowb + chunk * 16u;
+  return o ^ (((o >> 7) & (rowb / 16u - 1u)) << 4);
+}
+
 // Walks the tiles of one CTA (t = first, first + cps, ...) keeping (image, tile row, tile column) incrementally
 // instead of two integer divisions per tile and role.
 struct TileIter {
@@ -200,8 +214,14 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   // one it wants (a stage shared by both warpgroups would, with one or an odd number of stages).
   const int g = warp >> 2;
   const int wq = warp & 3;  // warp of the warpgroup: rows 16 wq .. 16 wq + 15 of each 64-row half
-  // the previous kernel may still be reading the buffer we store to (ping-pong) and ResConv layers read the residual
-  // from global memory: every storing / loading thread orders itself after the previous grid
+  const int px = lane >> 2;             // tile column of this thread's accumulator rows
+  const int c2 = 2 * (lane & 3);        // first of this thread's two columns in every 8-column block
+  // the CTA's output-channel slice is fixed: its shift values stay in registers for the whole launch
+  float2 sh[N / 8];
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) sh[j] = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
+  // the previous kernel may still be reading the buffer we store to (ping-pong) and ring ResConv layers read the
+  // residual from global memory: every storing / loading thread orders itself after the previous grid
   asm volatile("griddepcontrol.wait;" ::: "memory");
   mbar_wait(bar_w, 0);
   const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);  // LBO(=1) | start address, 16-byte units
@@ -220,8 +240,13 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   };
   advance((uint32_t)g * per_tile);
   const float slope = (p.epi_mode == EPI_BIAS) ? 1.f : 0.2f;  // max(a, slope * a): LeakyReLU(0.2), or no activation
-  const int px = lane >> 2;             // tile column of this thread's accumulator rows
-  const int c2 = 2 * (lane & 3);        // first of this thread's two columns in every 8-column block
+  // TMA-stored outputs: each warpgroup packs its tile into its own staging tile, [box][16 x 8 pixels][kBoxC channels]
+  // swizzled like the box rows, and one thread stores it as N / kBoxC tensor boxes
+  constexpr int kBoxC = store_box_c(N);
+  constexpr uint32_t kBoxRow = 2u * kBoxC, kBoxBytes = (uint32_t)(kTileH * kTileW) * kBoxRow;
+  const bool tma_out = !LAST && p.out_stage_bytes != 0;
+  const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for the warpgroup's bulk groups
+  const uint32_t out_smem = smem_base + p.off_out + (uint32_t)g * p.out_stage_bytes;
   float acc[2][N / 2];
 
   TileIter it(p, first + g * tstep, kMmaGroups * tstep);
@@ -251,32 +276,144 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
       issue_window<N, T>(p, acc, a_lo0 + stage * stage_units, b_lo0, 0u);
       wgmma_commit();
       wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);  // window free once the MMAs have read it
-      advance((uint32_t)kMmaGroups);
+      if (!residual) {  // window free once the MMAs have read it (ResConv reads its residual from it first)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);
+      }
     }
     acc_fence(acc[0]);
     acc_fence(acc[1]);
 
-    // ---- epilogue straight from the accumulator registers: d[h][4 j + 2 e + c] = tile row 8 h + 2 wq + e, column
-    // 8 j + c2 + c
+    // ---- epilogue from the accumulator registers: d[h][4 j + 2 e + c] = tile row 8 h + 2 wq + e, column 8 j + c2 + c
     const int b = it.b;
+    const int gy0 = it.ty * kTileH, gx0 = it.tx * kTileW;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        acc[h][4 * j] += sh[j].x;
+        acc[h][4 * j + 1] += sh[j].y;
+        acc[h][4 * j + 2] += sh[j].x;
+        acc[h][4 * j + 3] += sh[j].y;
+      }
+    if (residual && !RING) {
+      // the residual is the centre of the tile's staged window, still held: channel n of window pixel
+      // (y - halo_y0, x - halo_x0), read as 8 x 8 (pixel, channel) matrices straight into the accumulator layout
+      const uint32_t win = a_smem + stage * p.stage_bytes;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e - p.halo_y0) * p.halo_w + (lane & 7) - p.halo_x0);
+#pragma unroll
+          for (int jb = 0; jb < N / 8; jb += 4) {
+            const bool x4 = N / 8 - jb >= 4;  // N / 8 is even: an x2 tail at most
+            const int ch = n0 + 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
+            const int kb = ch >> 6;
+            const uint32_t rowb = (has_tail && kb == p.nkb - 1) ? 64u : 128u;
+            const uint32_t addr = win + p.kb_off[kb] + swz_off(pix, (uint32_t)(ch & 63) >> 3, rowb);
+            uint32_t r[4];
+            if (x4)
+              ldsm_x4(addr, r);
+            else
+              ldsm_x2(addr, r);
+#pragma unroll
+            for (int i = 0; i < (x4 ? 4 : 2); ++i) {
+              const float2 rf = Pack2<T>::unpack(r[i]);
+              acc[h][4 * (jb + i) + 2 * e] += rf.x;
+              acc[h][4 * (jb + i) + 2 * e + 1] += rf.y;
+            }
+          }
+        }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);
+    }
+    if (residual && RING) {  // ring slots are recycled before the epilogue: the residual comes from global memory
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int gy = gy0 + 8 * h + 2 * wq + e, gx = gx0 + px;
+          if (gy >= p.H || gx >= p.W) continue;
+          const T* rrow = reinterpret_cast<const T*>(p.in) + (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.cin + n0 + c2;
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) {
+            const float2 rf = Pack2<T>::unpack(__ldg(reinterpret_cast<const unsigned int*>(rrow + 8 * j)));
+            acc[h][4 * j + 2 * e] += rf.x;
+            acc[h][4 * j + 2 * e + 1] += rf.y;
+          }
+        }
+    }
+    if (!RING) advance((uint32_t)kMmaGroups);
+
+    if (tma_out) {
+      if (leader) bulk_wait_read<0>();  // the previous tile's stores have read the staging tile
+      named_bar_sync(1 + g, 128);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e) * kTileW + (lane & 7));
+#pragma unroll
+          for (int jb = 0; jb < N / 8; jb += 4) {
+            const bool x4 = N / 8 - jb >= 4;
+            const int col = 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
+            const uint32_t addr =
+                out_smem + (uint32_t)(col / kBoxC) * kBoxBytes + swz_off(pix, (uint32_t)(col % kBoxC) >> 3, kBoxRow);
+            uint32_t r[4];
+#pragma unroll
+            for (int i = 0; i < (x4 ? 4 : 2); ++i) {
+              const float a0 = acc[h][4 * (jb + i) + 2 * e], a1 = acc[h][4 * (jb + i) + 2 * e + 1];
+              r[i] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+            }
+            if (x4)
+              stsm_x4(addr, r);
+            else
+              stsm_x2(addr, r);
+          }
+        }
+      fence_proxy_async();  // the generic-proxy staging writes before the TMA engine reads them
+      named_bar_sync(1 + g, 128);
+      if (leader) {
+#pragma unroll
+        for (int s = 0; s < N / kBoxC; ++s)
+          tma_store_4d(&p.tm_out, out_smem + (uint32_t)s * kBoxBytes, n0 + s * kBoxC, gx0, gy0, b);
+        bulk_commit();
+      }
+      continue;
+    }
+
+    // ---- direct stores: lastconv's fp32 planes and the space-to-depth / sub-pixel patch forms
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int gy = it.ty * kTileH + 8 * h + 2 * wq + e, gx = it.tx * kTileW + px;
+        const int gy = gy0 + 8 * h + 2 * wq + e, gx = gx0 + px;
         if (gy >= p.H || gx >= p.W) continue;
         if (LAST) {
           // column n = c5*16 + pos: component c5 (4 flow + mask) of sub-pixel pos = y4*4 + x4 of this cell's 4x4 patch
           const int Hs = p.H * 4, Ws = p.W * 4;
+          if (N == 80) {
+            // all 80 columns in this CTA (n0 = 0): columns j = 2 c5 + s of this thread hold component c5 of sub-pixels
+            // (y4, x4) = (2 s + c2 / 4, c2 % 4 + c), so it writes whole float4 flow texels and float2 mask pairs
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+              const size_t o = ((size_t)b * Hs + (gy * 4 + 2 * s + (c2 >> 2))) * Ws + gx * 4 + (c2 & 3);
+#pragma unroll
+              for (int c = 0; c < 2; ++c)
+                p.out_flow[o + c] = make_float4(acc[h][4 * s + 2 * e + c], acc[h][4 * (2 + s) + 2 * e + c],
+                                                acc[h][4 * (4 + s) + 2 * e + c], acc[h][4 * (6 + s) + 2 * e + c]);
+              *reinterpret_cast<float2*>(p.out_mask + o) =
+                  make_float2(acc[h][4 * (8 + s) + 2 * e], acc[h][4 * (8 + s) + 2 * e + 1]);
+            }
+            continue;
+          }
 #pragma unroll
           for (int j = 0; j < N / 8; ++j) {
             const int n = n0 + 8 * j + c2;
-            const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + n));
             const int c5 = n >> 4, pos = n & 15;  // n even: n + 1 is the next sub-pixel of the same patch row
             const size_t o = ((size_t)b * Hs + (gy * 4 + (pos >> 2))) * Ws + gx * 4 + (pos & 3);
-            const float v0 = acc[h][4 * j + 2 * e] + sh.x, v1 = acc[h][4 * j + 2 * e + 1] + sh.y;
+            const float v0 = acc[h][4 * j + 2 * e], v1 = acc[h][4 * j + 2 * e + 1];
             if (c5 < 4) {
               float* f = reinterpret_cast<float*>(p.out_flow + o);
               f[c5] = v0;
@@ -288,17 +425,10 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
         } else {
           const bool patch = (p.out_s2d == 2);
           T* orow = reinterpret_cast<T*>(p.out) + out_pixel_offset(p, b, gy, gx);
-          const T* rrow = reinterpret_cast<const T*>(p.in) + (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.cin;
 #pragma unroll
           for (int j = 0; j < N / 8; ++j) {
             const int n = n0 + 8 * j + c2;
-            const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + n));
-            float a0 = acc[h][4 * j + 2 * e] + sh.x, a1 = acc[h][4 * j + 2 * e + 1] + sh.y;
-            if (residual) {
-              const float2 rf = Pack2<T>::unpack(__ldg(reinterpret_cast<const unsigned int*>(rrow + n)));
-              a0 += rf.x;
-              a1 += rf.y;
-            }
+            const float a0 = acc[h][4 * j + 2 * e], a1 = acc[h][4 * j + 2 * e + 1];
             // patch form: columns n = sub-pixel (n >> 3) x channel (n & 7)
             const size_t off = patch ? ((size_t)((n >> 3) >> 2) * (size_t)(4 * p.W) + (size_t)((n >> 3) & 3)) * 8 + (n & 7)
                                      : (size_t)n;
@@ -307,6 +437,7 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
         }
       }
   }
+  if (tma_out && leader) bulk_wait<0>();  // the CTA's last stores have landed before it exits
 }
 
 #endif  // VFI_HOST_EMU
@@ -501,14 +632,23 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   }
   p.b_hi = (1024u >> 4) | kDescSw128;  // B: SBO = 8 rows x 128 B, SWIZZLE_128B
   p.off_w = align_up(kCtrlBytes, 1024);
-  p.off_a = align_up(p.off_w + p.w_bytes, 1024);
+  // 16-bit NHWC outputs leave through TMA tensor stores from one staging tile per MMA warpgroup (128 cells x n_cta
+  // channels, 1024-aligned store boxes).  A dedicated region rather than the consumed window stage: the stage is free
+  // for the next fill as soon as the residual is read, and ring slots are recycled before the epilogue runs.  The
+  // staging costs window stages; a layer left with fewer than kMinStagedStages keeps direct stores (on H100 at 1080p
+  // the c = 128 ring ResConv with 2 slots instead of 3 and conv0.1 at c = 96 / 192 lost more than the stores gained).
+  constexpr int kMinStagedStages = 3;
+  auto fit = [&](uint32_t out_stage) {
+    p.out_stage_bytes = out_stage;
+    p.off_out = align_up(p.off_w + p.w_bytes, 1024);
+    p.off_a = p.off_out + kMmaGroups * out_stage;
+    for (int s = kMaxStages; s >= 1; --s)
+      if (p.off_a + (uint32_t)s * p.stage_bytes <= (uint32_t)kSmemLimit) return s;
+    return 0;
+  };
   int stages = 0;
-  for (int s = kMaxStages; s >= 1; --s) {
-    if (p.off_a + (uint32_t)s * p.stage_bytes <= (uint32_t)kSmemLimit) {
-      stages = s;
-      break;
-    }
-  }
+  if (L.epi_mode != EPI_LASTCONV && L.out_s2d == 0) stages = fit((uint32_t)(kTileH * kTileW) * L.n_cta * 2u);
+  if (stages < kMinStagedStages) stages = fit(0u);
   p.stages = stages;
   p.smem_bytes = p.off_a + (uint32_t)stages * p.stage_bytes;  // stage sizes are multiples of 1024
   return stages;
@@ -563,6 +703,13 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     if (L.cin < 64) p.tm64 = p.tm32;  // a single 32-channel k-block: the 64-channel map is never used
   } else {
     p.tm32 = p.tm64;
+  }
+  if (p.out_stage_bytes) {
+    const int bc = store_box_c(L.n_cta);
+    const CUtensorMapSwizzle swz = bc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                   : bc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                              : CU_TENSOR_MAP_SWIZZLE_32B;
+    if (!make_tmap(&p.tm_out, dt, out, L.n_total, W, H, B, bc, kTileW, kTileH, swz)) return cudaErrorInvalidValue;
   }
   // cps persistent CTAs per output-channel split
   int cps = num_sms / L.nsplit;

@@ -50,6 +50,7 @@ constexpr int kMaxK16 = 108;   // 9 taps x 192/16
 struct alignas(64) TapConvParams {
   CUtensorMap tm64;      // input as a {C, W, H, B} tensor with a {64 ch, halo_w, halo_h, 1} box, SWIZZLE_128B
   CUtensorMap tm32;      // same with a {32 ch, ...} box, SWIZZLE_64B (only used when cin % 64 == 32)
+  CUtensorMap tm_out;    // out_stage_bytes != 0: the output as {n_total, W, H, B}, box {store_box_c(n_cta), 8, 16, 1} (tapconv.cu)
   const void* in;        // [B, H, W, cin] 16-bit, NHWC
   void* out;             // [B, H, W, n_total] 16-bit NHWC; out_s2d = 1: its space-to-depth form; out_s2d = 2: the 4x4
                          // sub-pixel patch form [B, 4H, 4W, 8] with column n = (py*4 + px)*8 + ch (arch 4.26 lastconv features)
@@ -70,6 +71,7 @@ struct alignas(64) TapConvParams {
   uint32_t b_hi;                  // high word of the weight (B) descriptors
   uint32_t w_bytes;               // packed weight bytes of one split
   uint32_t off_w, off_a, stage_bytes, smem_bytes;
+  uint32_t off_out, out_stage_bytes;  // per-warpgroup staging tiles of the TMA output stores (0: direct stores)
   int nkb;                        // k-blocks of the staged window: 64 channels each, 32-channel tail if cin%64==32
   uint32_t kb_off[kMaxKBlocks];   // byte offset of each k-block inside a stage (1024-aligned)
   uint32_t tx_bytes;              // bytes one stage fill delivers (mbarrier transaction count)
