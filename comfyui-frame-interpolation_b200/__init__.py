@@ -1,4 +1,4 @@
-"""H100-native drop-in for the RIFE (and FILM) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
+"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
 
 Exports the same mapping names ComfyUI discovers in the reference's root __init__.py:23-47.
 """
@@ -6,12 +6,14 @@ from .node import RIFE_VFI, MakeInterpolationStateList, FloatToInt, Interpolatio
 from .film_node import FILM_VFI  # noqa: F401
 from .sepconv_node import SepconvVFI  # noqa: F401
 from .gmfss_node import GMFSS_Fortuna_VFI  # noqa: F401
+from .flavr_node import FLAVR_VFI  # noqa: F401
 
 NODE_CLASS_MAPPINGS = {
     "RIFE VFI": RIFE_VFI,
     "FILM VFI": FILM_VFI,
     "Sepconv VFI": SepconvVFI,
     "GMFSS Fortuna VFI": GMFSS_Fortuna_VFI,
+    "FLAVR VFI": FLAVR_VFI,
     "Make Interpolation State List": MakeInterpolationStateList,
     "VFI FloatToInt": FloatToInt,
 }
@@ -21,4 +23,5 @@ NODE_DISPLAY_NAME_MAPPINGS = {
     "FILM VFI": "FILM VFI (H100 native)",
     "Sepconv VFI": "Sepconv VFI (H100 native)",
     "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native)",
+    "FLAVR VFI": "FLAVR VFI (H100 native)",
 }

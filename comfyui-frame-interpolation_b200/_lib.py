@@ -15,6 +15,8 @@ SYMBOLS = [
     "vfi_film_load", "vfi_film_forward", "vfi_film_debug_set_ref", "vfi_film_debug_conv", "vfi_film_layer_plan",
     "vfi_film_last_macs", "vfi_film_debug_pack_host",
     "vfi_sepconv_load", "vfi_sepconv_forward", "vfi_sepconv_debug_set_ref", "vfi_sepconv_debug_pack_host",
+    "vfi_flavr_load", "vfi_flavr_forward", "vfi_flavr_debug_set_ref", "vfi_flavr_debug_conv", "vfi_flavr_layer_plan",
+    "vfi_flavr_info",
     # GMFSS building blocks (argtypes are set by gmfss.Ops)
     "vfi_gm_conv2d", "vfi_gm_conv2d_packed", "vfi_gm_transpose", "vfi_gm_convt4", "vfi_gm_instance_norm", "vfi_gm_layer_norm", "vfi_gm_softmax_rows", "vfi_gm_gemm", "vfi_gm_window", "vfi_gm_nchw_tokens", "vfi_gm_add_position", "vfi_gm_local_match", "vfi_gm_local_prop", "vfi_gm_convex_up", "vfi_gm_warp_zeros", "vfi_gm_resize", "vfi_gm_metric_input", "vfi_gm_pixel_shuffle2", "vfi_gm_axpby", "vfi_gm_copy_slice",
 ]
@@ -75,6 +77,12 @@ def lib():
     L.vfi_sepconv_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, vp, vp]
     L.vfi_sepconv_debug_set_ref.argtypes = [vp, i32]
     L.vfi_sepconv_debug_pack_host.argtypes = [i32, i32, i32, i32, i32, vp, vp, i64] + [C.POINTER(i32)] * 3
+    L.vfi_flavr_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]
+    L.vfi_flavr_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, vp, vp]
+    L.vfi_flavr_debug_set_ref.argtypes = [vp, i32]
+    L.vfi_flavr_debug_conv.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, vp]
+    L.vfi_flavr_layer_plan.argtypes = [vp, i32, vp, i32]
+    L.vfi_flavr_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     for name in SYMBOLS:
         if name not in ("vfi_last_error", "vfi_version", "vfi_launch_count", "vfi_film_last_macs"):
             getattr(L, name).restype = i32

@@ -160,12 +160,14 @@ struct vfi_ctx {
   std::vector<ProfSpan> prof_spans;  // pinned staging rings of the host-pointer path (pageable caller memory)
   vfi::FilmState* film = nullptr;  // FILM weights and workspace (film.cu)
   vfi::SepState* sep = nullptr;    // Sepconv weights and workspace (sepconv.cu)
+  vfi::ModelState* flavr = nullptr;  // FLAVR weights and workspace (flavr.cu)
 };
 
 namespace vfi {
 CtxInfo ctx_info(::vfi_ctx* c) { return CtxInfo{c->device, c->num_sms, c->s_h2d, c->s_comp, c->s_d2h}; }
 FilmState*& ctx_film(::vfi_ctx* c) { return c->film; }
 SepState*& ctx_sep(::vfi_ctx* c) { return c->sep; }
+ModelState*& ctx_flavr(::vfi_ctx* c) { return c->flavr; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi
 
@@ -680,6 +682,8 @@ int vfi_destroy(vfi_ctx* c) {
   cudaDeviceSynchronize();
   free_weights(c);
   film_destroy(c->film);
+  delete c->flavr;
+  c->flavr = nullptr;
   c->film = nullptr;
   sepconv_destroy(c->sep);
   c->sep = nullptr;

@@ -1,5 +1,6 @@
 // streamconv: implicit-GEMM convolution with STREAMED weights on the Hopper tensor cores (wgmma / TMA / mbarrier),
-// sm_90a only.  The conv kernel of the FILM path (SURVEY.md section 8 row a10).
+// sm_90a only.  The conv kernel of the FILM path (SURVEY.md section 8 row a10), of the Sepconv trunk and of FLAVR, whose
+// 3-D convolutions add a temporal tap axis: the A producer walks (temporal tap, k-block) pairs (see src_image).
 //
 // Replaces the cuDNN / ATen kernels behind film_arch.conv (film_arch.py:784-798: Conv2d(k x k, padding='same')
 // [+ LeakyReLU(0.2)], k = 1, 2, 3) for every layer of
@@ -54,7 +55,7 @@ constexpr uint32_t kSConsumerArrivals = 4 * kSMmaGroups;
 struct TileCoord {
   int b, ty, tx;
 };
-// tile index -> (image, tile row, tile column); tiles past the end map to image B: TMA zero-fills, nothing is stored
+// tile index -> (output image, tile row, tile column); tiles past the end map to image B: nothing is stored
 __device__ __forceinline__ TileCoord tile_coord(const StreamConvParams& p, int tile) {
   TileCoord c;
   if (tile >= p.ntiles) {
@@ -69,6 +70,14 @@ __device__ __forceinline__ TileCoord tile_coord(const StreamConvParams& p, int t
   c.ty = rem / p.tiles_x;
   c.tx = rem - c.ty * p.tiles_x;
   return c;
+}
+
+// input image that temporal tap dt of output image b reads: images are (sample, plane) pairs, b = s * T_out + t_out,
+// and the tap reads plane t_out + dt - pad_t of the same sample.  A plane outside [0, T_in) and the images of tiles past
+// the end map to image B_in, one past the end of the input tensor: TMA zero-fills it, the checker skips it.
+__device__ __forceinline__ int src_image(const StreamConvParams& p, int b, int dt) {
+  const int s = b / p.T_out, pl = b - s * p.T_out + dt - p.pad_t;
+  return (b >= p.B || pl < 0 || pl >= p.T_in) ? p.B_in : s * p.T_in + pl;
 }
 
 __device__ __forceinline__ void ring_next(uint32_t& slot, uint32_t& ph, uint32_t n) {
@@ -130,7 +139,8 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
         TileCoord tc[2];
         tc[0] = tile_coord(p, pass * mt);
         tc[1] = tile_coord(p, pass * mt + 1);
-        for (int kb = 0; kb < p.nkb; ++kb) {
+        for (int j = 0; j < p.kt * p.nkb; ++j) {  // (temporal tap, k-block), the order of the packed weights
+          const int dt = j / p.nkb, kb = j - dt * p.nkb;
           mbar_wait(bar_aempty + 8 * slot, ph ^ 1u);
           mbar_arrive_expect_tx(bar_afull + 8 * slot, (uint32_t)mt * p.a_tx_bytes);
           const bool s0 = kb < p.nkb0;
@@ -138,7 +148,7 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
           const int c0 = (s0 ? kb : kb - p.nkb0) * 64;
           for (int t = 0; t < mt; ++t)
             tma_load_4d(a_smem + slot * p.a_slot_bytes + (uint32_t)t * p.a_win_bytes, tm, bar_afull + 8 * slot, c0,
-                        tc[t].tx * kTileW + p.halo_x0, tc[t].ty * kTileH + p.halo_y0, tc[t].b);
+                        tc[t].tx * kTileW + p.halo_x0, tc[t].ty * kTileH + p.halo_y0, src_image(p, tc[t].b, dt));
           ring_next(slot, ph, (uint32_t)p.a_slots);
         }
       }
@@ -150,7 +160,7 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
     if (lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_split_bytes;
       uint32_t slot = 0, ph = 0;
-      const int per_pass = p.nkb * p.ntaps;
+      const int per_pass = p.kt * p.nkb * p.ntaps;
       for (int k = 0; k < my_passes; ++k) {
         for (int j = 0; j < per_pass; ++j) {
           mbar_wait(bar_bempty + 8 * slot, ph ^ 1u);
@@ -182,7 +192,7 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
     // MMAs of one (k-block, tap) form one wgmma group; the slot of the previous group is released once it completes
     uint32_t prev_b = 0, prev_a = 0;
     bool prev_last_tap = false, have_prev = false;
-    for (int kb = 0; kb < p.nkb; ++kb) {
+    for (int kb = 0; kb < p.kt * p.nkb; ++kb) {
       mbar_wait(bar_afull + 8 * aslot, aph);
       for (int tap = 0; tap < p.ntaps; ++tap) {
         mbar_wait(bar_bfull + 8 * bslot, bph);
@@ -296,19 +306,23 @@ __global__ void streamconv_ref_kernel(const __grid_constant__ StreamConvParams p
     const int split = n / p.n_cta, nl = n - split * p.n_cta;
     const T* w = reinterpret_cast<const T*>(reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_split_bytes);
     float acc = 0.f;
-    for (int kb = 0; kb < p.nkb; ++kb) {
-      const bool s0 = kb < p.nkb0;
-      const T* src = reinterpret_cast<const T*>(s0 ? p.src[0] : p.src[1]);
-      const int pitch = s0 ? p.src_pitch[0] : p.src_pitch[1];
-      const int c0 = (s0 ? kb : kb - p.nkb0) * 64;
-      for (int tap = 0; tap < p.ntaps; ++tap) {
-        const int y = gy + p.halo_y0 + tap / p.ksize, x = gx + p.halo_x0 + tap % p.ksize;
-        if (y < 0 || y >= p.H || x < 0 || x >= p.W) continue;
-        const T* px = src + (((size_t)b * p.H + y) * p.W + x) * (size_t)pitch + c0;
-        const T* wr = w + ((size_t)(kb * p.ntaps + tap) * p.n_cta + nl) * 64;
-        for (int c = 0; c < 64; ++c) {
-          const int chunk = c >> 3;
-          acc = fmaf(sc_ld<T>(px + c), sc_ld<T>(wr + ((chunk ^ (nl & 7)) * 8 + (c & 7))), acc);
+    for (int dt = 0; dt < p.kt; ++dt) {
+      const int img = src_image(p, b, dt);
+      if (img >= p.B_in) continue;
+      for (int kb = 0; kb < p.nkb; ++kb) {
+        const bool s0 = kb < p.nkb0;
+        const T* src = reinterpret_cast<const T*>(s0 ? p.src[0] : p.src[1]);
+        const int pitch = s0 ? p.src_pitch[0] : p.src_pitch[1];
+        const int c0 = (s0 ? kb : kb - p.nkb0) * 64;
+        for (int tap = 0; tap < p.ntaps; ++tap) {
+          const int y = gy + p.halo_y0 + tap / p.ksize, x = gx + p.halo_x0 + tap % p.ksize;
+          if (y < 0 || y >= p.H || x < 0 || x >= p.W) continue;
+          const T* px = src + (((size_t)img * p.H + y) * p.W + x) * (size_t)pitch + c0;
+          const T* wr = w + ((size_t)((dt * p.nkb + kb) * p.ntaps + tap) * p.n_cta + nl) * 64;
+          for (int c = 0; c < 64; ++c) {
+            const int chunk = c >> 3;
+            acc = fmaf(sc_ld<T>(px + c), sc_ld<T>(wr + ((chunk ^ (nl & 7)) * 8 + (c & 7))), acc);
+          }
         }
       }
     }
@@ -366,11 +380,18 @@ uint32_t sc_align_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
 bool streamconv_plan(const StreamConvLayer& L, StreamConvParams* pp) {
   StreamConvParams& p = *pp;
   if (L.ksize < 1 || L.ksize > 3 || L.c0 % 64 || L.c1 % 64 || L.c0 < 64 || L.n_total % 16 || L.n_total < 16) return false;
+  if (L.kt < 1 || L.kt > 4 || L.pad_t < 0 || L.T_in < 1 || L.T_out < 1) return false;
   p.ksize = L.ksize;
   p.ntaps = L.ksize * L.ksize;
   // padding='same': (k-1)/2 before, the rest after (film_arch.py:789); L.pad_before >= 0 overrides it (Sepconv's stride-2
-  // convs run as 2x2 convs over a space-to-depth input with their one padding row / column BEFORE)
-  p.halo_y0 = p.halo_x0 = -(L.pad_before >= 0 ? L.pad_before : (L.ksize - 1) / 2);
+  // convs run as 2x2 convs over a space-to-depth input with their one padding row / column BEFORE); L.pad_before_x >= 0
+  // sets the columns apart from the rows (the phases of a transposed conv, flavr.cu)
+  p.halo_y0 = -(L.pad_before >= 0 ? L.pad_before : (L.ksize - 1) / 2);
+  p.halo_x0 = L.pad_before_x >= 0 ? -L.pad_before_x : p.halo_y0;
+  p.kt = L.kt;
+  p.pad_t = L.pad_t;
+  p.T_in = L.T_in;
+  p.T_out = L.T_out;
   p.halo_h = kTileH + L.ksize - 1;
   p.halo_w = kTileW + L.ksize - 1;
   p.nkb0 = L.c0 / 64;
@@ -384,7 +405,7 @@ bool streamconv_plan(const StreamConvLayer& L, StreamConvParams* pp) {
   p.nsplit = L.n_total / n_cta;
   p.mt = kSMmaGroups;  // one tile per MMA warpgroup
   p.b_slot_bytes = (uint32_t)n_cta * 128u;
-  p.w_split_bytes = (size_t)p.nkb * p.ntaps * p.b_slot_bytes;
+  p.w_split_bytes = (size_t)p.kt * p.nkb * p.ntaps * p.b_slot_bytes;
   p.a_tx_bytes = (uint32_t)p.halo_w * (uint32_t)p.halo_h * 128u;
   p.a_win_bytes = sc_align_up(p.a_tx_bytes, 1024);
   p.a_slot_bytes = (uint32_t)p.mt * p.a_win_bytes;
@@ -422,28 +443,36 @@ static uint16_t to_op(float v, int op_type) {
   return u;
 }
 
-// Host-only operand packer (film.cu, sepconv.cu): wfun(output column n, tap = ky * k + kx, padded input channel) -> weight;
-// layout [split][k-block][tap][n_cta rows][64 channels = 128 B, 16-byte chunks XOR (row & 7)] = what one B slot receives.
-bool pack_streamconv(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int)>& wfun,
-                     std::vector<uint16_t>* out, StreamConvParams* plan) {
+// Host-only operand packer (flavr.cu): wfun(output column n, temporal tap dt, tap = ky * k + kx, padded input channel) ->
+// weight; layout [split][dt][k-block][tap][n_cta rows][64 channels = 128 B, 16-byte chunks XOR (row & 7)] = what one B
+// slot receives, in the order the B producer streams them.
+bool pack_streamconv3d(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int, int)>& wfun,
+                       std::vector<uint16_t>* out, StreamConvParams* plan) {
   StreamConvParams& p = *plan;
   p = StreamConvParams{};
   if (!streamconv_plan(L, &p)) return false;
   const int ntaps = L.ksize * L.ksize;
-  const size_t per_split = (size_t)p.nkb * ntaps * p.n_cta * 64;
+  const size_t per_split = (size_t)L.kt * p.nkb * ntaps * p.n_cta * 64;
   std::vector<uint16_t>& pk = *out;
   pk.assign((size_t)p.nsplit * per_split, 0);
   for (int sp = 0; sp < p.nsplit; ++sp)
-    for (int kb = 0; kb < p.nkb; ++kb)
-      for (int tap = 0; tap < ntaps; ++tap)
-        for (int nl = 0; nl < p.n_cta; ++nl) {
-          uint16_t* row = &pk[sp * per_split + ((size_t)(kb * ntaps + tap) * p.n_cta + nl) * 64];
-          for (int c = 0; c < 64; ++c) {
-            const float val = wfun(sp * p.n_cta + nl, tap, kb * 64 + c);
-            if (val != 0.f) row[(((c >> 3) ^ (nl & 7)) * 8) + (c & 7)] = to_op(val, op_type);
+    for (int dt = 0; dt < L.kt; ++dt)
+      for (int kb = 0; kb < p.nkb; ++kb)
+        for (int tap = 0; tap < ntaps; ++tap)
+          for (int nl = 0; nl < p.n_cta; ++nl) {
+            uint16_t* row = &pk[sp * per_split + ((size_t)((dt * p.nkb + kb) * ntaps + tap) * p.n_cta + nl) * 64];
+            for (int c = 0; c < 64; ++c) {
+              const float val = wfun(sp * p.n_cta + nl, dt, tap, kb * 64 + c);
+              if (val != 0.f) row[(((c >> 3) ^ (nl & 7)) * 8) + (c & 7)] = to_op(val, op_type);
+            }
           }
-        }
   return true;
+}
+
+// 2-D form (film.cu, sepconv.cu): wfun(output column n, tap = ky * k + kx, padded input channel) -> weight
+bool pack_streamconv(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int)>& wfun,
+                     std::vector<uint16_t>* out, StreamConvParams* plan) {
+  return pack_streamconv3d(L, op_type, [&](int n, int, int tap, int j) { return wfun(n, tap, j); }, out, plan);
 }
 
 cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void* src0, int pitch0, const void* src1,
@@ -478,16 +507,17 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
   }
   p.w = L.w;
   p.shift = L.shift;
-  p.B = B;
+  p.B = B * L.T_out;
+  p.B_in = B * L.T_in;
   p.H = H;
   p.W = W;
   p.tiles_y = (H + kTileH - 1) / kTileH;
   p.tiles_x = (W + kTileW - 1) / kTileW;
-  p.ntiles = B * p.tiles_y * p.tiles_x;
+  p.ntiles = p.B * p.tiles_y * p.tiles_x;
   p.npasses = (p.ntiles + p.mt - 1) / p.mt;
 
   if (use_ref) {
-    const size_t total = (size_t)B * H * W * L.n_total;
+    const size_t total = (size_t)p.B * H * W * L.n_total;
     const int blocks = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
     if (op_type == OP_BF16)
       VFI_LAUNCH(streamconv_ref_kernel<__nv_bfloat16>, blocks, 256, 0, st, p);
@@ -501,9 +531,9 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
 #else
 
   const CUtensorMapDataType dt = (op_type == OP_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  if (!make_slice_tmap(&p.tm[0], dt, src0, L.c0, pitch0, W, H, B, p.halo_w, p.halo_h)) return cudaErrorInvalidValue;
+  if (!make_slice_tmap(&p.tm[0], dt, src0, L.c0, pitch0, W, H, p.B_in, p.halo_w, p.halo_h)) return cudaErrorInvalidValue;
   if (L.c1) {
-    if (!make_slice_tmap(&p.tm[1], dt, src1, L.c1, pitch1, W, H, B, p.halo_w, p.halo_h)) return cudaErrorInvalidValue;
+    if (!make_slice_tmap(&p.tm[1], dt, src1, L.c1, pitch1, W, H, p.B_in, p.halo_w, p.halo_h)) return cudaErrorInvalidValue;
   } else {
     p.tm[1] = p.tm[0];
   }

@@ -168,6 +168,8 @@ cudaError_t launch_sepconv(const float* in, const float* ver, const float* hor, 
 // ---------------------------------------------------------------------------------------------
 // streamconv (streamconv.cu): k x k 'same' convolution with streamed weights - the FILM conv kernel.
 //   out[b, y, x, n] = act( bias[n] + sum_{tap, c} in[b, y+dy, x+dx, c] * W[tap, c, n] ),  in = cat(src0[:c0], src1[:c1])
+// With kt > 1 it is a kt x k x k 3-D convolution over [sample][plane][H][W][C] tensors (FLAVR, flavr.cu): output plane t
+// sums temporal taps dt = 0 .. kt-1 of input plane t + dt - pad_t (zero outside [0, T_in)).
 // ---------------------------------------------------------------------------------------------
 struct StreamConvLayer {
   int ksize = 3;          // 1, 2 or 3; padding='same' (film_arch.py:784-790)
@@ -177,7 +179,10 @@ struct StreamConvLayer {
   int ext = 0;            // 1: Sepconv epilogue instead: PReLU with one learned `slope` (1.0 = none), then + residual
   float slope = 1.f;
   int pad_before = -1;    // rows / columns of zero padding before the window; -1: (ksize - 1) / 2 ('same')
-  void* w = nullptr;      // device, packed [split][k-block][tap][n_cta][64 ch, 16-byte chunks XOR (n & 7)] 16-bit
+  int pad_before_x = -1;  // columns of zero padding before the window when >= 0 (rows keep pad_before)
+  int kt = 1, pad_t = 0;  // temporal taps and zero planes before plane 0
+  int T_in = 1, T_out = 1;  // planes per sample of the input / output (the launch's B counts samples)
+  void* w = nullptr;      // device, packed [split][dt][k-block][tap][n_cta][64 ch, 16-byte chunks XOR (n & 7)] 16-bit
   float* shift = nullptr; // device, [n_total] bias
 };
 
@@ -193,7 +198,9 @@ struct alignas(64) StreamConvParams {
   const void* w;
   const float* shift;
   size_t w_split_bytes;   // packed weight bytes of one output-channel split
-  int B, H, W;
+  int B, H, W;            // B: output images (samples x T_out)
+  int B_in;               // input images (samples x T_in)
+  int kt, pad_t, T_in, T_out;
   int ksize, ntaps, nkb0, nkb;
   int n_total, n_cta, nsplit, act;
   int halo_y0, halo_x0, halo_h, halo_w;
@@ -214,6 +221,9 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
 // host-only operand packer (film.cu): wfun(output column n, tap = ky * k + kx, padded input channel) -> weight
 bool pack_streamconv(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int)>& wfun,
                      std::vector<uint16_t>* out, StreamConvParams* plan);
+// the same with temporal taps (flavr.cu): wfun(output column n, temporal tap dt, tap, padded input channel) -> weight
+bool pack_streamconv3d(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int, int)>& wfun,
+                       std::vector<uint16_t>* out, StreamConvParams* plan);
 
 // ---- Sepconv element-wise kernels (sepconv_elem.cu) ----
 struct SepPairIdx {  // source frames of every pair of a pass
@@ -260,6 +270,26 @@ cudaError_t launch_film_flow_head(int op_type, const void* x, int pitch, int C, 
 cudaError_t launch_film_out_rgb(int op_type, const void* x, int pitch, const float* w, const float* bias, int clamp01,
                                 float* out, int B, int H, int W, cudaStream_t st);
 
+// ---- FLAVR kernels around the convolutions (flavr_elem.cu); images = windows x 4 planes ----
+constexpr int kFlavrMaxWindows = 8;
+struct FlavrFrameIdx {  // source frame of every image of a pass (window k, plane t at k * 4 + t)
+  int i[4 * kFlavrMaxWindows];
+};
+cudaError_t launch_flavr_frame_sums(const float* frames, int cstride, const FlavrFrameIdx& idx, int n_img, int H, int W,
+                                    int Hp, int Wp, int pt, int pl, float* sums, cudaStream_t st);
+cudaError_t launch_flavr_prep(const float* frames, int cstride, const FlavrFrameIdx& idx, int n_img, int T, int H, int W,
+                              int Hp, int Wp, int pt, int pl, const float* sums, float4* out, cudaStream_t st);
+cudaError_t launch_flavr_stem(int op_type, const float4* xin, int n_img, int T, int Hp, int Wp, const float* w,
+                              const float* bias, void* out, cudaStream_t st);
+int flavr_sum_chunks(size_t npx);  // partial sums per sample of chan_sums (a function of the geometry only)
+cudaError_t launch_flavr_chan_sums(int op_type, const void* x, int C, size_t npx, int S, float* partial, cudaStream_t st);
+cudaError_t launch_flavr_gate(const float* partial, size_t npx, int groups, int C, size_t count, const float* w,
+                              const float* b, int S, float* g, cudaStream_t st);
+cudaError_t launch_flavr_apply(int op_type, const void* x, int phases, const float* g, const void* res, int act, void* out,
+                               void* s2d, int C, int n_img, int T, int H, int W, cudaStream_t st);
+cudaError_t launch_flavr_outconv(int op_type, const void* x, int S, int Hp, int Wp, int H, int W, int pt, int pl,
+                                 const float* w, const float* bias, const float* sums, int T, float* out, cudaStream_t st);
+
 cudaError_t launch_adacof(const float* in, const float* weight, const float* off_i, const float* off_j, float* out, int N,
                           int C, int Hin, int Win, int F, int dil, int Ho, int Wo, cudaStream_t st);
 cudaError_t launch_edt_pass(const float* data, float* out, int bs, int h, int w, float diam2, cudaStream_t st);
@@ -268,6 +298,10 @@ void set_error(const std::string& s);
 
 // ---- context access for film.cu (vfi_ctx is defined in rife46.cu) ----
 struct FilmState;
+// state that a model's .cu file keeps in a context; vfi_destroy deletes it through this base
+struct ModelState {
+  virtual ~ModelState() = default;
+};
 struct CtxInfo {
   int device, num_sms;
   cudaStream_t s_h2d, s_comp, s_d2h;
@@ -277,6 +311,7 @@ void film_destroy(FilmState* f);  // film.cu
 
 CtxInfo ctx_info(::vfi_ctx* c);
 FilmState*& ctx_film(::vfi_ctx* c);
+ModelState*& ctx_flavr(::vfi_ctx* c);  // a FlavrState (flavr.cu)
 SepState*& ctx_sep(::vfi_ctx* c);
 void ctx_add_launches(::vfi_ctx* c, int n);
 

@@ -391,3 +391,104 @@ class SepconvEngine:
 
     def sync(self):
         check(self._L.vfi_sync(self._ctx))
+
+
+# ------------------------------------------------------------------------------------------------- FLAVR
+def flavr_state_dict_names(enc_bias: bool = False):
+    """UNet_3D_3D("unet_18", 4, n_outputs).state_dict() order (flavr_arch.py:134-164, resnet_3D.py:118-151); the
+    encoder convs carry a bias only in the 4x / 8x checkpoints (resnet_3D.useBias)."""
+    names = ["encoder.stem.0.weight"] + (["encoder.stem.0.bias"] if enc_bias else [])
+    for l in range(1, 5):
+        for b in range(2):
+            p = f"encoder.layer{l}.{b}."
+            for conv in ("conv1", "conv2"):
+                names += [p + conv + ".0.weight"] + ([p + conv + ".0.bias"] if enc_bias else [])
+            names += [p + "fg.attn_layer.0.weight", p + "fg.attn_layer.0.bias"]
+            if b == 0 and l > 1:
+                names.append(p + "downsample.0.weight")
+    for d in range(5):
+        m = "upconv" if d in (1, 2, 4) else "conv"
+        names += [f"decoder.{d}.{m}.0.weight", f"decoder.{d}.{m}.0.bias", f"decoder.{d}.{m}.1.attn_layer.0.weight",
+                  f"decoder.{d}.{m}.1.attn_layer.0.bias"]
+    return names + ["feature_fuse.conv.0.weight", "outconv.1.weight", "outconv.1.bias"]
+
+
+class FlavrEngine:
+    """FLAVR (FLAVR_2x.pth / FLAVR_4x.pth / FLAVR_8x.pth) on one H100: `state_dict` = UNet_3D_3D's, keys without the
+    `module.` prefix.  Whether the encoder convs carry a bias and how many outputs the model has are read from the
+    state dict; only output 0 is computed (the node uses no other)."""
+
+    MAX_WINDOWS = 8
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, dtype: str = "float32"):
+        if not torch.cuda.is_available():
+            raise VfiError("no CUDA device: this path has no CPU fallback")
+        if dtype not in OPERAND:
+            raise ValueError(f"dtype must be one of {list(OPERAND)}")
+        self._L = lib()
+        self.device = int(device)
+        self._ctx = C.c_void_p()
+        check(self._L.vfi_create(self.device, C.byref(self._ctx)))
+        names = flavr_state_dict_names("encoder.stem.0.bias" in state_dict)
+        missing = [n for n in names if n not in state_dict]
+        if missing:
+            raise KeyError(f"state_dict is not a FLAVR checkpoint; missing {missing[:3]} ...")
+        hold = [state_dict[n].detach().to("cpu", torch.float32).contiguous() for n in names]
+        ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+        numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+        check(self._L.vfi_flavr_load(self._ctx, ptrs, numel, len(hold), OPERAND[dtype]))
+        n_out, eb = C.c_int(), C.c_int()
+        check(self._L.vfi_flavr_info(self._ctx, C.byref(n_out), C.byref(eb)))
+        self.n_outputs, self.enc_bias = n_out.value, bool(eb.value)
+        self.dtype = dtype
+
+    def close(self):
+        if getattr(self, "_ctx", None) is not None and self._ctx.value:
+            self._L.vfi_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def forward(self, frames: torch.Tensor, first: Sequence[int], out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """frames: CUDA float32 [N,H,W,C>=3] NHWC -> CUDA float32 [len(first),H,W,3]: for window k (frames first[k] ..
+        first[k] + 3) the model's first output on the padded frames, cropped (not clamped)."""
+        assert frames.is_cuda and frames.dtype == torch.float32 and frames.is_contiguous() and frames.dim() == 4
+        n, h, w, c = frames.shape
+        fa = _i32(first)
+        nw = len(fa)
+        assert 1 <= nw <= self.MAX_WINDOWS
+        if out is None:
+            out = torch.empty((nw, h, w, 3), dtype=torch.float32, device=frames.device)
+        assert out.is_cuda and out.is_contiguous() and out.dtype == torch.float32 and tuple(out.shape) == (nw, h, w, 3)
+        st = torch.cuda.current_stream(frames.device).cuda_stream
+        check(self._L.vfi_flavr_forward(self._ctx, frames.data_ptr(), n, h, w, c, fa.ctypes.data, nw, out.data_ptr(), st))
+        return out
+
+    # ------------------------------------------------------------------ hooks
+    def set_ref(self, use_ref: bool):
+        check(self._L.vfi_flavr_debug_set_ref(self._ctx, 1 if use_ref else 0))
+
+    def debug_conv(self, layer, src0, src1, out, n_windows, H, W, impl=0, pitch0=None, pitch1=None, out_pitch=None):
+        st = torch.cuda.current_stream(src0.device).cuda_stream
+        check(self._L.vfi_flavr_debug_conv(
+            self._ctx, layer, src0.data_ptr(), int(pitch0 if pitch0 is not None else src0.shape[-1]),
+            None if src1 is None else src1.data_ptr(), 0 if src1 is None else int(pitch1 if pitch1 is not None else src1.shape[-1]),
+            out.data_ptr(), int(out_pitch if out_pitch is not None else out.shape[-1]), n_windows, H, W, impl, st))
+        return out
+
+    def layer_plan(self, layer):
+        v = np.zeros(16, np.int32)
+        check(self._L.vfi_flavr_layer_plan(self._ctx, layer, v.ctypes.data, 16))
+        keys = ("c0", "c1", "n_total", "ksize", "kt", "pad_t", "T_in", "T_out", "pad_y", "pad_x", "n_cta", "nsplit",
+                "a_slots", "b_slots", "smem_bytes", "ext")
+        return dict(zip(keys, [int(x) for x in v]))
+
+    def launch_count(self) -> int:
+        return int(self._L.vfi_launch_count(self._ctx))
+
+    def sync(self):
+        check(self._L.vfi_sync(self._ctx))

@@ -179,6 +179,31 @@ int vfi_sepconv_debug_set_ref(vfi_ctx* ctx, int use_ref);
 int vfi_sepconv_debug_pack_host(int stride2, int cin, int cout, int n_total, int operand_type, const float* w, uint16_t* out,
                                 int64_t out_cap, int* c0, int* n_cta, int* nsplit);
 
+/* FLAVR (`FLAVR VFI` node: UNet_3D_3D "unet_18", 4 input frames) ---------------------------------------- */
+#define VFI_FLAVR_NUM_TENSORS 59       /* UNet_3D_3D.state_dict() without encoder conv biases (FLAVR_2x.pth) */
+#define VFI_FLAVR_NUM_TENSORS_BIAS 76  /* with them (FLAVR_4x.pth, FLAVR_8x.pth: resnet_3D.useBias) */
+#define VFI_FLAVR_MAX_WINDOWS 8
+/* Replaces: build_flavr(path) - flavr/__init__.py:14-23.  HOST float32 arrays in UNet_3D_3D.state_dict() order (engine.py
+ * flavr_state_dict_names); the tensor count tells whether the encoder convs carry a bias, the size of outconv.1.weight
+ * the number of outputs (3 x n_outputs channels; only output 0 is used).  Sizes are checked. */
+int vfi_flavr_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type);
+/* Replaces: `model([f0, f1, f2, f3])[0]` on the InputPadder(16)-padded frames + padder.unpad (flavr/__init__.py:67-84,
+ * :110) for n_windows windows: window k reads frames first_frame[k] .. first_frame[k] + 3.  DEVICE pointers: frames
+ * [n_frames, H, W, C] float32 NHWC (C >= 3, first three channels read), out [n_windows, H, W, 3] float32 NHWC (not
+ * clamped, like the reference); first_frame: HOST array.  Asynchronous on `stream`. */
+int vfi_flavr_forward(vfi_ctx* ctx, const float* frames, int n_frames, int H, int W, int C, const int32_t* first_frame,
+                      int n_windows, float* out, void* stream);
+/* Test hooks: every conv through the CUDA-core checker (1) / the wgmma kernel (0); run one conv layer (id: encoder
+ * 10 * layer + 3 * block + {0 conv1, 1 conv2, 2 downsample}; decoder 40 + 4 * d + phase; 60 feature_fuse) on caller
+ * tensors [n_windows * T_in][H][W][pitch] 16-bit -> [n_windows * T_out][H][W][out_pitch]; its plan as
+ * {c0, c1, n_total, ksize, kt, pad_t, T_in, T_out, pad_y, pad_x, n_cta, nsplit, a_slots, b_slots, smem_bytes, ext};
+ * the loaded checkpoint's n_outputs and encoder-bias flag. */
+int vfi_flavr_debug_set_ref(vfi_ctx* ctx, int use_ref);
+int vfi_flavr_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0, const void* src1, int pitch1, void* out,
+                         int out_pitch, int n_windows, int H, int W, int impl, void* stream);
+int vfi_flavr_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
+int vfi_flavr_info(vfi_ctx* ctx, int* n_outputs, int* enc_bias);
+
 /* Test / profiling hooks (used by tests/ and bench.py only) --------------------------------------------- */
 /* Run ONE convolution layer of block `block` (0..3; arch 4.26: 0..4): layer 0 = conv0.0, 1 = conv0.1, 2..9 = ResConv
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
