@@ -115,6 +115,18 @@ __device__ __forceinline__ void stsm_x4(uint32_t addr, const uint32_t* r) {
 __device__ __forceinline__ void stsm_x2(uint32_t addr, const uint32_t* r) {
   asm volatile("stmatrix.sync.aligned.m8n8.x2.shared.b16 [%0], {%1, %2};" ::"r"(addr), "r"(r[0]), "r"(r[1]) : "memory");
 }
+// transposed forms: thread t holds column t / 4, rows 2 (t % 4), +1 of matrix i in register i (low half: the even row)
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t* r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stsm_x4_t(uint32_t addr, const uint32_t* r) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma (Hopper warpgroup MMA)
 // Shared-memory matrix descriptor (PTX ISA "Matrix Descriptor Format" of wgmma): start address >> 4 [0,14), leading byte

@@ -514,10 +514,12 @@ int run_encode(vfi_ctx* c, const Geometry& g, int f, int n, cudaStream_t st) {
     const int Hh = g.Hp / 2, Wh = g.Wp / 2;
     const size_t fbytes = c->arch == 417 ? 16 : 8;  // feature bytes per full-resolution pixel
     LAUNCH(launch_head0(c->op_type, imgs, c->enc[0], c->enc[1], c->hA.p, n, g.Hp, g.Wp, st));
-    LAUNCH(launch_tapconv(c->head[0], c->op_type, c->hA.p, c->hB.p, nullptr, nullptr, n, Hh, Wh, c->num_sms, false, st));
-    LAUNCH(launch_tapconv(c->head[1], c->op_type, c->hB.p, c->hA.p, nullptr, nullptr, n, Hh, Wh, c->num_sms, false, st));
+    LAUNCH(launch_tapconv(c->head[0], c->op_type, c->hA.p, c->hB.p, nullptr, nullptr, n, Hh, Wh, c->num_sms,
+                          TAPCONV_PLANNED, st));
+    LAUNCH(launch_tapconv(c->head[1], c->op_type, c->hB.p, c->hA.p, nullptr, nullptr, n, Hh, Wh, c->num_sms,
+                          TAPCONV_PLANNED, st));
     LAUNCH(launch_tapconv(c->head[2], c->op_type, c->hA.p, (uint8_t*)c->feats.p + (size_t)f * px * fbytes, nullptr, nullptr,
-                          n, Hh, Wh, c->num_sms, false, st));
+                          n, Hh, Wh, c->num_sms, TAPCONV_PLANNED, st));
   }
   return VFI_OK;
 }
@@ -598,27 +600,27 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
     span_end();
     span_begin(10 * i + 1);
     LAUNCH(launch_tapconv(c->layers[i][0], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, B, Hs / 2, Ws / 2,
-                          c->num_sms, false, st));
+                          c->num_sms, TAPCONV_PLANNED, st));
     span_end();
     span_begin(10 * i + 2);
     LAUNCH(launch_tapconv(c->layers[i][1], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, B, Hs / 4, Ws / 4,
-                          c->num_sms, false, st));
+                          c->num_sms, TAPCONV_PLANNED, st));
     span_end();
     void* a = c->featA.p;
     void* b = c->featB.p;
     span_begin(10 * i + 3);
     for (int j = 0; j < 8; ++j) {
       LAUNCH(launch_tapconv(c->layers[i][2 + j], c->op_type, a, b, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
-                            false, st));
+                            TAPCONV_PLANNED, st));
       std::swap(a, b);
     }
     span_end();
     span_begin(10 * i + 4);
     LAUNCH(launch_tapconv(c->layers[i][10], c->op_type, a, nullptr, fs.f[i], fs.m[i], B, Hs / 4, Ws / 4, c->num_sms,
-                          false, st));
+                          TAPCONV_PLANNED, st));
     if (c->arch == 426 && i + 1 < nb)  // the 8 feature channels of lastconv, for the next block's input
       LAUNCH(launch_tapconv(c->layers[i][11], c->op_type, a, c->tE[i].p, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
-                            false, st));
+                            TAPCONV_PLANNED, st));
     if (g.k[i] > 1) {  // the up-scaled block's output goes straight back onto the dense planes
       LAUNCH(launch_fold_down(fs.f[i], fs.m[i], g.k[i], F, M, B, g.Hp, g.Wp, fs.mask_replace, st));
       lo = i + 1;
@@ -1393,14 +1395,16 @@ int vfi_rife46_debug_layer(vfi_ctx* c, int block, int layer, const void* in, voi
   if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
   if (block >= num_blocks(c->arch) || layer > 11 || (layer == 11 && (c->arch != 426 || block + 1 >= num_blocks(c->arch))))
     return fail(VFI_E_INVALID, "no such block / layer in the loaded arch");
+  if (impl != TAPCONV_PLANNED && impl != TAPCONV_CHECKER && impl != TAPCONV_CELL_MAJOR)
+    return fail(VFI_E_INVALID, "impl must be 0 (tensor cores), 1 (checker) or 2 (tensor cores, cell-major MMAs)");
   CK(cudaSetDevice(c->device));
   const TapConvLayer& L = c->layers[block][layer];
   if (layer == 10) {
     if (!out_mask) return fail(VFI_E_INVALID, "lastconv needs out_mask");
-    LAUNCH(launch_tapconv(L, c->op_type, in, nullptr, (float4*)out, (float*)out_mask, B, H, W, c->num_sms, impl == 1,
+    LAUNCH(launch_tapconv(L, c->op_type, in, nullptr, (float4*)out, (float*)out_mask, B, H, W, c->num_sms, impl,
                           (cudaStream_t)stream));
   } else {
-    LAUNCH(launch_tapconv(L, c->op_type, in, out, nullptr, nullptr, B, H, W, c->num_sms, impl == 1,
+    LAUNCH(launch_tapconv(L, c->op_type, in, out, nullptr, nullptr, B, H, W, c->num_sms, impl,
                           (cudaStream_t)stream));
   }
   return VFI_OK;
@@ -1433,7 +1437,7 @@ int vfi_rife46_debug_state(vfi_ctx* c, float* flow4_out, float* mask_out, int ba
 }
 
 int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
-                          int64_t* macs_per_cell) {
+                          int64_t* macs_per_cell, int* cmajor) {
   if (!c || block < 0 || layer < 0) return fail(VFI_E_INVALID, "bad argument");
   if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
   if (block >= num_blocks(c->arch) || layer > 11 || (layer == 11 && (c->arch != 426 || block + 1 >= num_blocks(c->arch))))
@@ -1446,6 +1450,7 @@ int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_
   if (nsplit) *nsplit = L.nsplit;
   if (smem_bytes) *smem_bytes = (int)p.smem_bytes;
   if (macs_per_cell) *macs_per_cell = (int64_t)L.ktotal16 * 16 * L.n_total;
+  if (cmajor) *cmajor = p.cmajor;
   return VFI_OK;
 }
 

@@ -16,6 +16,16 @@
 // once (x1.41 halo), not 9x as with im2col.  Weights of the CTA's output-channel slice are resident in shared memory
 // for the whole launch (one bulk copy, already in the swizzled operand layout).
 //
+// Channel-major MMAs (p.cmajor, template CM: non-ring 3 x 3 convs over 64 input channels with n_cta = 64 and a staged
+// 16-bit NHWC output).  The
+// operand roles swap: the packed weights are byte for byte a K-major SWIZZLE_128B A operand (64 output-channel rows)
+// and the window a K-major B operand whose 8-row groups are the tile's 16 rows of 8 cells (SBO = halo_w * 128 B), so
+// ONE m64n128k16 per K=16 step computes the whole tile.  Per step shared memory then supplies 2 KB of weights + 4 KB of
+// window instead of 2 x (2 KB + 2 KB): with cells on M and N = 64 the two MMAs alone need all of an SM's shared-memory
+// bandwidth at the tensor peak (128 B/clk against 1/16 B per MAC), channel-major three quarters of it.  Same products
+// in the same K order into fp32: the outputs are bit-identical to the cell-major form (DESIGN.md section 5 has the
+// measured gain).
+//
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles):
 //   warpgroups 0, 1 : MMA + epilogue.  Warpgroup w takes the CTA's tiles w, w + 2, ... and keeps the whole tile's
 //                     accumulators (2 x 64 rows x n_cta columns, fp32) in registers, so one warpgroup's epilogue
@@ -44,6 +54,7 @@ struct Ctrl {
 constexpr uint32_t kCtrlBytes = 256;
 constexpr int kMmaGroups = 2, kTmaWarp = 8, kThreads = 128 * kMmaGroups + 32;
 static_assert(sizeof(Ctrl) <= kCtrlBytes, "control block");
+constexpr int kCmRuns = 9, kCmRunLen = 4;  // channel-major MMA issue: 9 taps x 4 K=16 steps (64 input channels)
 
 __device__ __forceinline__ size_t out_pixel_offset(const TapConvParams& p, int b, int gy, int gx) {
   // element offset of channel 0 of grid cell (b, gy, gx) in the output tensor
@@ -103,10 +114,26 @@ struct TileIter {
 
 // One window's MMAs for both 64-row halves of the tile: p.nruns runs of p.run_len consecutive K=16 steps (same tap,
 // same k-block: both descriptors advance by 32 bytes per step).  a_base / b_base: start-address words (16-byte units,
-// LBO = 1) of the window and of the weights of this k-block.
-template <int N, typename T>
+// LBO = 1) of the window and of the weights of this k-block.  CM: one m64n128 per step, weights as A and the window as
+// B; its accumulator d[4 j + 2 h + c] (tile row j = 0..15) is acc[j / 8][4 (j % 8) + 2 h + c].  The channel-major
+// layers are 3 x 3 convs over 64 channels (tapconv_plan: kCmRuns runs of kCmRunLen steps), so their 36 MMAs are issued
+// as straight-line code: with no loop back-edge between them ptxas keeps them one chain behind a single
+// warpgroup.arrive instead of injecting an arrive in front of every MMA and ending each one's scoreboard group.
+template <int N, bool CM, typename T>
 __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc)[2][N / 2], uint32_t a_base,
                                              uint32_t b_base, uint32_t accumulate_first) {
+  if constexpr (CM) {
+#pragma unroll
+    for (int r = 0; r < kCmRuns; ++r) {
+      const uint4 d = p.mma[r];
+      const uint64_t w64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b_base + d.z);
+      const uint64_t x64 = ((uint64_t)d.y << 32) | (uint64_t)(a_base + d.x);
+#pragma unroll
+      for (int i = 0; i < kCmRunLen; ++i)
+        wgmma_ss<128, T>(&acc[0][0], w64 + 2u * i, x64 + 2u * i, (r | i) ? 1u : accumulate_first);
+    }
+    return;
+  }
 #pragma unroll 1
   for (int r = 0; r < p.nruns; ++r) {
     const uint4 d = p.mma[r];
@@ -125,8 +152,9 @@ __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc
   }
 }
 
-template <typename T, bool RING, bool LAST, int N>
+template <typename T, bool RING, bool LAST, int N, bool CM>
 __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_constant__ TapConvParams p) {
+  static_assert(!CM || (N == 64 && !RING && !LAST), "channel-major: 64 output channels, staged window, 16-bit output");
   extern __shared__ __align__(1024) uint8_t smem[];
   // Programmatic dependent launch (launch_tapconv sets the attribute): the next kernel in the stream may start its
   // CTAs as soon as every CTA of this grid has passed this point, i.e. while our last tiles are still running - they do
@@ -216,10 +244,16 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   const int wq = warp & 3;  // warp of the warpgroup: rows 16 wq .. 16 wq + 15 of each 64-row half
   const int px = lane >> 2;             // tile column of this thread's accumulator rows
   const int c2 = 2 * (lane & 3);        // first of this thread's two columns in every 8-column block
-  // the CTA's output-channel slice is fixed: its shift values stay in registers for the whole launch
-  float2 sh[N / 8];
+  // the CTA's output-channel slice is fixed: its shift values stay in registers for the whole launch (channel-major:
+  // this thread's two channels 16 wq + lane / 4, +8)
+  float2 sh[CM ? 1 : N / 8];
+  if constexpr (CM) {
+    const int ch = n0 + 16 * wq + (lane >> 2);
+    sh[0] = make_float2(__ldg(p.shift + ch), __ldg(p.shift + ch + 8));
+  } else {
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) sh[j] = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
+    for (int j = 0; j < N / 8; ++j) sh[j] = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
+  }
   // the previous kernel may still be reading the buffer we store to (ping-pong) and ring ResConv layers read the
   // residual from global memory: every storing / loading thread orders itself after the previous grid
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -244,7 +278,7 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   // swizzled like the box rows, and one thread stores it as N / kBoxC tensor boxes
   constexpr int kBoxC = store_box_c(N);
   constexpr uint32_t kBoxRow = 2u * kBoxC, kBoxBytes = (uint32_t)(kTileH * kTileW) * kBoxRow;
-  const bool tma_out = !LAST && p.out_stage_bytes != 0;
+  const bool tma_out = CM || (!LAST && p.out_stage_bytes != 0);  // (channel-major layers always stage their output)
   const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for the warpgroup's bulk groups
   const uint32_t out_smem = smem_base + p.off_out + (uint32_t)g * p.out_stage_bytes;
   float acc[2][N / 2];
@@ -256,7 +290,7 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
       for (int kb = 0; kb < p.nkb; ++kb) {
         wait_full();
         wgmma_fence();
-        issue_window<N, T>(p, acc, a_lo0 + stage * stage_units, b_lo0 + (uint32_t)kb * b_kb, kb > 0 ? 1u : 0u);
+        issue_window<N, CM, T>(p, acc, a_lo0 + stage * stage_units, b_lo0 + (uint32_t)kb * b_kb, kb > 0 ? 1u : 0u);
         wgmma_commit();
         if (kb > 0) {  // the previous slot's MMAs have read it
           wgmma_wait<1>();
@@ -273,7 +307,7 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
     } else {
       wait_full();
       wgmma_fence();
-      issue_window<N, T>(p, acc, a_lo0 + stage * stage_units, b_lo0, 0u);
+      issue_window<N, CM, T>(p, acc, a_lo0 + stage * stage_units, b_lo0, 0u);
       wgmma_commit();
       wgmma_wait<0>();
       if (!residual) {  // window free once the MMAs have read it (ResConv reads its residual from it first)
@@ -285,46 +319,82 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
     acc_fence(acc[1]);
 
     // ---- epilogue from the accumulator registers: d[h][4 j + 2 e + c] = tile row 8 h + 2 wq + e, column 8 j + c2 + c
+    // channel-major: acc[jh][4 jl + 2 h + c] = channel 16 wq + lane / 4 + 8 h of tile row 8 jh + jl, column c2 + c
     const int b = it.b;
     const int gy0 = it.ty * kTileH, gx0 = it.tx * kTileW;
+    if constexpr (CM) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+      for (int jh = 0; jh < 2; ++jh)
 #pragma unroll
-      for (int j = 0; j < N / 8; ++j) {
-        acc[h][4 * j] += sh[j].x;
-        acc[h][4 * j + 1] += sh[j].y;
-        acc[h][4 * j + 2] += sh[j].x;
-        acc[h][4 * j + 3] += sh[j].y;
-      }
+        for (int jl = 0; jl < 8; ++jl) {
+          acc[jh][4 * jl] += sh[0].x;
+          acc[jh][4 * jl + 1] += sh[0].x;
+          acc[jh][4 * jl + 2] += sh[0].y;
+          acc[jh][4 * jl + 3] += sh[0].y;
+        }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          acc[h][4 * j] += sh[j].x;
+          acc[h][4 * j + 1] += sh[j].y;
+          acc[h][4 * j + 2] += sh[j].x;
+          acc[h][4 * j + 3] += sh[j].y;
+        }
+    }
     if (residual && !RING) {
       // the residual is the centre of the tile's staged window, still held: channel n of window pixel
       // (y - halo_y0, x - halo_x0), read as 8 x 8 (pixel, channel) matrices straight into the accumulator layout
       const uint32_t win = a_smem + stage * p.stage_bytes;
+      if constexpr (CM) {
+        // transposed reads: matrix i = lane / 8 is tile row 8 jh + 2 jp + i / 2 (8 cells) x channels 16 wq + 8 (i % 2)
+        const int i = lane >> 3;
+        const int ch = n0 + 16 * wq + 8 * (i & 1);
+        const int kb = ch >> 6;
+        const uint32_t rowb = (has_tail && kb == p.nkb - 1) ? 64u : 128u;
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+        for (int jh = 0; jh < 2; ++jh)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e - p.halo_y0) * p.halo_w + (lane & 7) - p.halo_x0);
-#pragma unroll
-          for (int jb = 0; jb < N / 8; jb += 4) {
-            const bool x4 = N / 8 - jb >= 4;  // N / 8 is even: an x2 tail at most
-            const int ch = n0 + 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
-            const int kb = ch >> 6;
-            const uint32_t rowb = (has_tail && kb == p.nkb - 1) ? 64u : 128u;
-            const uint32_t addr = win + p.kb_off[kb] + swz_off(pix, (uint32_t)(ch & 63) >> 3, rowb);
+          for (int jp = 0; jp < 4; ++jp) {
+            const int row = 8 * jh + 2 * jp + (i >> 1);
+            const uint32_t pix = (uint32_t)((row - p.halo_y0) * p.halo_w + (lane & 7) - p.halo_x0);
             uint32_t r[4];
-            if (x4)
-              ldsm_x4(addr, r);
-            else
-              ldsm_x2(addr, r);
+            ldsm_x4_t(win + p.kb_off[kb] + swz_off(pix, (uint32_t)(ch & 63) >> 3, rowb), r);
 #pragma unroll
-            for (int i = 0; i < (x4 ? 4 : 2); ++i) {
-              const float2 rf = Pack2<T>::unpack(r[i]);
-              acc[h][4 * (jb + i) + 2 * e] += rf.x;
-              acc[h][4 * (jb + i) + 2 * e + 1] += rf.y;
+            for (int q = 0; q < 4; ++q) {
+              const float2 rf = Pack2<T>::unpack(r[q]);
+              acc[jh][4 * (2 * jp + (q >> 1)) + 2 * (q & 1)] += rf.x;
+              acc[jh][4 * (2 * jp + (q >> 1)) + 2 * (q & 1) + 1] += rf.y;
             }
           }
-        }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e - p.halo_y0) * p.halo_w + (lane & 7) - p.halo_x0);
+#pragma unroll
+            for (int jb = 0; jb < N / 8; jb += 4) {
+              const bool x4 = N / 8 - jb >= 4;  // N / 8 is even: an x2 tail at most
+              const int ch = n0 + 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
+              const int kb = ch >> 6;
+              const uint32_t rowb = (has_tail && kb == p.nkb - 1) ? 64u : 128u;
+              const uint32_t addr = win + p.kb_off[kb] + swz_off(pix, (uint32_t)(ch & 63) >> 3, rowb);
+              uint32_t r[4];
+              if (x4)
+                ldsm_x4(addr, r);
+              else
+                ldsm_x2(addr, r);
+#pragma unroll
+              for (int i = 0; i < (x4 ? 4 : 2); ++i) {
+                const float2 rf = Pack2<T>::unpack(r[i]);
+                acc[h][4 * (jb + i) + 2 * e] += rf.x;
+                acc[h][4 * (jb + i) + 2 * e + 1] += rf.y;
+              }
+            }
+          }
+      }
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);
     }
@@ -349,29 +419,49 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
     if (tma_out) {
       if (leader) bulk_wait_read<0>();  // the previous tile's stores have read the staging tile
       named_bar_sync(1 + g, 128);
+      if constexpr (CM) {
+        // transposed stores: matrix i = lane / 8 is tile row 8 jh + 2 jp + i / 2 x channels 16 wq + 8 (i % 2) (one box)
+        const int i = lane >> 3;
+        const uint32_t chunk = (uint32_t)(2 * wq + (i & 1));
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+        for (int jh = 0; jh < 2; ++jh)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e) * kTileW + (lane & 7));
-#pragma unroll
-          for (int jb = 0; jb < N / 8; jb += 4) {
-            const bool x4 = N / 8 - jb >= 4;
-            const int col = 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
-            const uint32_t addr =
-                out_smem + (uint32_t)(col / kBoxC) * kBoxBytes + swz_off(pix, (uint32_t)(col % kBoxC) >> 3, kBoxRow);
+          for (int jp = 0; jp < 4; ++jp) {
+            const uint32_t pix = (uint32_t)((8 * jh + 2 * jp + (i >> 1)) * kTileW + (lane & 7));
             uint32_t r[4];
 #pragma unroll
-            for (int i = 0; i < (x4 ? 4 : 2); ++i) {
-              const float a0 = acc[h][4 * (jb + i) + 2 * e], a1 = acc[h][4 * (jb + i) + 2 * e + 1];
-              r[i] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+            for (int q = 0; q < 4; ++q) {
+              const float a0 = acc[jh][4 * (2 * jp + (q >> 1)) + 2 * (q & 1)];
+              const float a1 = acc[jh][4 * (2 * jp + (q >> 1)) + 2 * (q & 1) + 1];
+              r[q] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
             }
-            if (x4)
-              stsm_x4(addr, r);
-            else
-              stsm_x2(addr, r);
+            stsm_x4_t(out_smem + swz_off(pix, chunk, kBoxRow), r);
           }
-        }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e) * kTileW + (lane & 7));
+#pragma unroll
+            for (int jb = 0; jb < N / 8; jb += 4) {
+              const bool x4 = N / 8 - jb >= 4;
+              const int col = 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
+              const uint32_t addr =
+                  out_smem + (uint32_t)(col / kBoxC) * kBoxBytes + swz_off(pix, (uint32_t)(col % kBoxC) >> 3, kBoxRow);
+              uint32_t r[4];
+#pragma unroll
+              for (int i = 0; i < (x4 ? 4 : 2); ++i) {
+                const float a0 = acc[h][4 * (jb + i) + 2 * e], a1 = acc[h][4 * (jb + i) + 2 * e + 1];
+                r[i] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+              }
+              if (x4)
+                stsm_x4(addr, r);
+              else
+                stsm_x2(addr, r);
+            }
+          }
+      }
       fence_proxy_async();  // the generic-proxy staging writes before the TMA engine reads them
       named_bar_sync(1 + g, 128);
       if (leader) {
@@ -651,16 +741,27 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   if (stages < kMinStagedStages) stages = fit(0u);
   p.stages = stages;
   p.smem_bytes = p.off_a + (uint32_t)stages * p.stage_bytes;  // stage sizes are multiples of 1024
+  // Channel-major MMAs (top of this file) need exactly 64 output channels for the M of one wgmma, the whole window
+  // held until the epilogue (its residual read) and the staging tile the transposed fragments are stored through.  The
+  // shared-memory plan is the same in both orientations.  VFI_TAPCONV_CMAJOR=0 keeps cells on M (A/B runs).
+  static const bool cmajor_on = [] {
+    const char* e = std::getenv("VFI_TAPCONV_CMAJOR");
+    return !(e && e[0] == '0');
+  }();
+  p.cmajor = (cmajor_on && !L.ring && L.n_cta == 64 && p.out_stage_bytes != 0 && p.nruns == kCmRuns &&
+              p.run_len == kCmRunLen) ? 1 : 0;
   return stages;
 }
 
 cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, void* out, float4* out_flow,
-                           float* out_mask, int B, int H, int W, int num_sms, bool use_ref, cudaStream_t st) {
+                           float* out_mask, int B, int H, int W, int num_sms, int impl, cudaStream_t st) {
   TapConvParams p{};
   if (tapconv_plan(L, &p) < 1) {
     set_error("tapconv: layer does not fit in shared memory");
     return cudaErrorInvalidConfiguration;
   }
+  if (impl == TAPCONV_CELL_MAJOR) p.cmajor = 0;
+  bool use_ref = impl == TAPCONV_CHECKER;
   if (L.out_s2d == 1 && ((H | W) & 1)) {
     set_error("tapconv: space-to-depth output needs even H and W");
     return cudaErrorInvalidValue;
@@ -745,13 +846,16 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
   auto pick_n = [&](auto tag, auto ring, auto lst) -> cudaError_t {
     using T = decltype(tag);
     constexpr bool R = decltype(ring)::value, LA = decltype(lst)::value;
+    if constexpr (!R && !LA) {
+      if (p.cmajor) return go(tapconv_kernel<T, false, false, 64, true>);  // (tapconv_plan: n_cta == 64)
+    }
     switch (L.n_cta) {  // tapconv_plan admits multiples of 16 up to 96
-      case 16: return go(tapconv_kernel<T, R, LA, 16>);
-      case 32: return go(tapconv_kernel<T, R, LA, 32>);
-      case 48: return go(tapconv_kernel<T, R, LA, 48>);
-      case 64: return go(tapconv_kernel<T, R, LA, 64>);
-      case 80: return go(tapconv_kernel<T, R, LA, 80>);
-      default: return go(tapconv_kernel<T, R, LA, 96>);
+      case 16: return go(tapconv_kernel<T, R, LA, 16, false>);
+      case 32: return go(tapconv_kernel<T, R, LA, 32, false>);
+      case 48: return go(tapconv_kernel<T, R, LA, 48, false>);
+      case 64: return go(tapconv_kernel<T, R, LA, 64, false>);
+      case 80: return go(tapconv_kernel<T, R, LA, 80, false>);
+      default: return go(tapconv_kernel<T, R, LA, 96, false>);
     }
   };
   auto pick = [&](auto tag) -> cudaError_t {

@@ -66,6 +66,7 @@ struct alignas(64) TapConvParams {
   int epi_mode, out_s2d;
   int nruns, run_len;    // MMA issue: nruns runs of run_len consecutive K=16 steps (mma[r] = first step of run r)
   int ring;              // 1: the window streams through a ring of single k-block slots (see tapconv.cu)
+  int cmajor;            // 1: channel-major MMAs, the 64 output channels on the wgmma M and the tile's 128 cells on N
   int tiles_x, tiles_y, ntiles;
   int ctas_per_split;
   uint32_t b_hi;                  // high word of the weight (B) descriptors
@@ -105,9 +106,11 @@ constexpr int kMaxBatch = 16;
 enum OperandType : int { OP_F16 = 0, OP_BF16 = 1 };
 
 // ---- launchers (defined in tapconv.cu / elementwise.cu) -------------------------------------
-// Returns cudaSuccess or the launch error; `use_ref` runs the CUDA-core checker instead of the tensor-core kernel.
+// Returns cudaSuccess or the launch error.  impl: 0 the tensor-core kernel as planned, 1 the CUDA-core checker, 2 the
+// tensor-core kernel with cells on the wgmma M even where the plan chose the channel-major MMAs (A/B comparisons).
+enum TapConvImpl : int { TAPCONV_PLANNED = 0, TAPCONV_CHECKER = 1, TAPCONV_CELL_MAJOR = 2 };
 cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, void* out, float4* out_flow,
-                           float* out_mask, int B, int H, int W, int num_sms, bool use_ref, cudaStream_t st);
+                           float* out_mask, int B, int H, int W, int num_sms, int impl, cudaStream_t st);
 // smem/stage plan for a layer (for DESIGN.md tables and tests); returns 0 stages when it cannot fit
 int tapconv_plan(const TapConvLayer& L, TapConvParams* p_out);
 

@@ -209,15 +209,17 @@ int vfi_flavr_info(vfi_ctx* ctx, int* n_outputs, int* enc_bias);
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
  * [B, 4H, 4W, 8] 16-bit.  `in`/`out` are device tensors in the kernel-native layouts documented in DESIGN.md
  * (16-bit NHWC; layers 0/1 read space-to-depth inputs; layer 10 writes float4 flow + float mask planes).
- * impl 0 = wgmma kernel, 1 = CUDA-core checker with the same packed weights. */
+ * impl 0 = wgmma kernel as planned, 1 = CUDA-core checker with the same packed weights, 2 = wgmma kernel with the
+ * grid cells on the MMA's M even where the plan runs the layer channel-major (see vfi_rife46_layer_plan). */
 int vfi_rife46_debug_layer(vfi_ctx* ctx, int block, int layer, const void* in, void* out, void* out_mask, int B, int H,
                            int W, int impl, void* stream);
 /* Copies the full-resolution flow (float4 [batch,Hp,Wp]) and mask (float [batch,Hp,Wp]) of the LAST internal
  * pass into caller-provided DEVICE buffers (either may be NULL to only query Hp/Wp); synchronises. */
 int vfi_rife46_debug_state(vfi_ctx* ctx, float* flow4_out, float* mask_out, int batch, int* Hp, int* Wp);
-/* Static plan of a layer for (block, layer): shared-memory stages, CTA output channels, splits, smem bytes. */
+/* Static plan of a layer for (block, layer): shared-memory stages, CTA output channels, splits, smem bytes, MACs per
+ * grid cell, and cmajor = 1 when the layer runs channel-major (output channels on the MMA's M, 128 cells on N). */
 int vfi_rife46_layer_plan(vfi_ctx* ctx, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
-                          int64_t* macs_per_cell);
+                          int64_t* macs_per_cell, int* cmajor);
 int vfi_sync(vfi_ctx* ctx);
 
 /* Measurement hook (bench.py's roofline lines): while enabled, every internal pass of the RIFE forward schedule records
