@@ -16,6 +16,28 @@ so the oracle is pinned against outputs of the reference itself, imported unmodi
 the build container by ``tools/make_golden.py``; the vectors live in ``tests/golden/``
 and ``tests/test_oracle_golden.py`` checks this file against them bit-for-bit-close
 (max abs 1e-6) on every CPU run.
+
+16-bit-faithful mode.  ``ifnet*_forward(..., operand="float16" | "bfloat16")`` (and ``ifblock``) evaluate the same
+graph in float64 and round to 16 bits exactly where the CUDA library stores or packs a 16-bit value, so that a
+comparison with the library measures accumulation order only.  With ``operand=None`` (the default) nothing is
+rounded and the fp32 graph above runs unchanged, bit for bit.  T is the operand type; where the library stores or
+packs each tensor (csrc/elementwise.cu, csrc/rife46.cu, csrc/tapconv.cu):
+
+| tensor | stored / packed by | type |
+|---|---|---|
+| frames, clamped to [0,1] and zero-padded (``imgs``) | ``prep_frames_kernel`` | fp32: read by encoders and ``final`` |
+| the same frames (``imgs_h``) | ``prep_frames_kernel`` | fp16 for either T: read by the block-input warps |
+| 4.7 encode Conv2d output (``e16``) | ``encode_conv_kernel``, fp32 weights | fp32 |
+| 4.7 encoded features f0 / f1 | ``encode_deconv_kernel``, fp32 weights | fp16 for either T |
+| 4.17 / 4.26 Head cnn0 output | ``head0_kernel``, fp32 weights | T |
+| 4.17 / 4.26 Head cnn1, cnn2 outputs | tapconv, weights round_T(w) | T |
+| 4.17 / 4.26 Head features f0 / f1 (cnn3) | tapconv, weights round_T(w) | T |
+| block input [warps, t, mask, (features), flow/s] after the 1/s resampling | ``front*`` / ``front_up*`` kernels, fp32 arithmetic | T |
+| conv0.0, conv0.1 outputs | tapconv, weights round_T(w), bias fp32 | T |
+| ResConv outputs | tapconv, weights round_T(w*beta) (product in fp32), shift bias*beta (fp32), residual = the T input | T |
+| lastconv flow (4) and mask (1) at the block's resolution | tapconv, weights round_T(w), bias fp32 | fp32 |
+| 4.26 lastconv feature channels 5..12 (layer 11) at the block's resolution | tapconv, weights round_T(w), bias fp32 | T |
+| accumulated flow / mask, final warps, sigmoid blend | ``flow_at``, ``fold_down``, ``final_kernel`` | fp32 |
 """
 from __future__ import annotations
 
@@ -113,6 +135,29 @@ def synthetic_state_dict(seed: int = 0, flow_gain: float = 1.0, beta_jitter: flo
 # --------------------------------------------------------------------------------------
 # model pieces
 # --------------------------------------------------------------------------------------
+_OPERAND = {"float16": torch.float16, "bfloat16": torch.bfloat16}
+
+
+def _dt(operand: Optional[str]):
+    if operand is not None and operand not in _OPERAND:
+        raise ValueError(f"operand must be None, 'float16' or 'bfloat16', not {operand!r}")
+    return None if operand is None else _OPERAND[operand]
+
+
+def q16(x: torch.Tensor, dt) -> torch.Tensor:
+    """``x`` rounded to the 16-bit type ``dt`` and widened to float64; ``x`` itself when ``dt`` is None."""
+    return x if dt is None else x.to(dt).to(torch.float64)
+
+
+def _wb(sd: Dict[str, torch.Tensor], prefix: str, dt, wdt="same"):
+    """(weight, bias) of ``prefix``: as stored when ``dt`` is None, else the weight rounded to ``wdt`` (``dt`` unless
+    given; None keeps fp32 - the CUDA-core encoders) and both widened to float64."""
+    w, b = sd[prefix + "weight"], sd[prefix + "bias"]
+    if dt is None:
+        return w, b
+    return q16(w, dt if wdt == "same" else wdt).double(), b.double()
+
+
 def warp(img: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     """Backward bilinear warp -- rife_arch.py:31-70.
 
@@ -121,8 +166,8 @@ def warp(img: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     ``grid_sample(bilinear, padding_mode="border", align_corners=True)`` (:64-70).
     """
     n, _, h, w = flow.shape
-    hor = torch.linspace(-1.0, 1.0, w).view(1, 1, 1, w).expand(n, -1, h, -1)
-    ver = torch.linspace(-1.0, 1.0, h).view(1, 1, h, 1).expand(n, -1, -1, w)
+    hor = torch.linspace(-1.0, 1.0, w, dtype=flow.dtype, device=flow.device).view(1, 1, 1, w).expand(n, -1, h, -1)
+    ver = torch.linspace(-1.0, 1.0, h, dtype=flow.dtype, device=flow.device).view(1, 1, h, 1).expand(n, -1, -1, w)
     grid = torch.cat([hor, ver], 1)
     fl = torch.cat(
         [flow[:, 0:1] / ((img.shape[3] - 1.0) / 2.0), flow[:, 1:2] / ((img.shape[2] - 1.0) / 2.0)], 1
@@ -141,35 +186,49 @@ def resconv(x, w, b, beta):
     return F.leaky_relu(F.conv2d(x, w, b, stride=1, padding=1) * beta + x, LRELU_SLOPE)
 
 
+def resconv_packed(sd: Dict[str, torch.Tensor], q: str, dt):
+    """The library's ResConv operands (csrc/rife46.cu build_resconv): (conv(x)+b)*beta == conv_{w*beta}(x) + b*beta, the
+    products w*beta and b*beta formed in fp32, w*beta rounded to ``dt``; returned in float64."""
+    beta = sd[q + "beta"].reshape(-1)
+    return q16(sd[q + "conv.weight"] * beta.view(-1, 1, 1, 1), dt).double(), (sd[q + "conv.bias"] * beta).double()
+
+
 def ifblock(sd: Dict[str, torch.Tensor], b: int, x: torch.Tensor, flow: Optional[torch.Tensor], scale: float,
-            taps: Optional[dict] = None):
+            taps: Optional[dict] = None, operand: Optional[str] = None):
     """IFBlock.forward for arch 4.6 -- rife_arch.py:237-276.
 
     down-scale x (and flow, also divided by scale) bilinearly with align_corners=False
     (:238-249), conv0 = two stride-2 conv+lrelu (:250), 8 ResConv (:254), lastconv =
     ConvTranspose2d(c,24,4,2,1) + PixelShuffle(2) (:215-218,:256), up-scale by ``scale``,
-    flow = ch0-3 * scale, mask = ch4 (:263-266,:275).
+    flow = ch0-3 * scale, mask = ch4 (:263-266,:275).  ``operand``: see the module docstring.
     """
+    dt = _dt(operand)
     p = f"block{b}."
     x = F.interpolate(x, scale_factor=1.0 / scale, mode="bilinear", align_corners=False)
     if flow is not None:
         flow = F.interpolate(flow, scale_factor=1.0 / scale, mode="bilinear", align_corners=False) * 1.0 / scale
         x = torch.cat((x, flow), 1)
+    x = q16(x, dt)
     if taps is not None:
         taps[f"b{b}.x"] = x
-    feat = conv_lrelu(x, sd[p + "conv0.0.0.weight"], sd[p + "conv0.0.0.bias"], 2)
+    feat = q16(conv_lrelu(x, *_wb(sd, p + "conv0.0.0.", dt), 2), dt)
     if taps is not None:
         taps[f"b{b}.c00"] = feat
-    feat = conv_lrelu(feat, sd[p + "conv0.1.0.weight"], sd[p + "conv0.1.0.bias"], 2)
+    feat = q16(conv_lrelu(feat, *_wb(sd, p + "conv0.1.0.", dt), 2), dt)
     if taps is not None:
         taps[f"b{b}.c01"] = feat
     for j in range(8):
         q = p + f"convblock.{j}."
-        feat = resconv(feat, sd[q + "conv.weight"], sd[q + "conv.bias"], sd[q + "beta"])
+        if dt is None:
+            feat = resconv(feat, sd[q + "conv.weight"], sd[q + "conv.bias"], sd[q + "beta"])
+        else:
+            feat = q16(F.leaky_relu(F.conv2d(feat, *resconv_packed(sd, q, dt), padding=1) + feat, LRELU_SLOPE), dt)
     if taps is not None:
         taps[f"b{b}.feat"] = feat
-    tmp = F.conv_transpose2d(feat, sd[p + "lastconv.0.weight"], sd[p + "lastconv.0.bias"], stride=2, padding=1)
+    tmp = F.conv_transpose2d(feat, *_wb(sd, p + "lastconv.0.", dt), stride=2, padding=1)
     tmp = F.pixel_shuffle(tmp, 2)
+    if tmp.shape[1] == 13 and dt is not None:  # arch 4.26: the 8 feature channels are stored in T, flow / mask in fp32
+        tmp = torch.cat((tmp[:, :5], q16(tmp[:, 5:], dt)), 1)
     if taps is not None:
         taps[f"b{b}.tmp"] = tmp
     tmp = F.interpolate(tmp, scale_factor=scale, mode="bilinear", align_corners=False)
@@ -178,8 +237,46 @@ def ifblock(sd: Dict[str, torch.Tensor], b: int, x: torch.Tensor, flow: Optional
     return tmp[:, :4] * scale, tmp[:, 4:5]
 
 
+def _prep(img0, img1, timestep, operand):
+    """clamp + zero-pad to x64 (rife_arch.py:476-485) and the timestep plane (:491-494).  Returns (img0, img1, t, the
+    frames the block inputs sample, dt): with an operand the fp32 frames widened to float64 and their fp16 copies."""
+    dt = _dt(operand)
+    if dt is not None:
+        img0, img1 = img0.double(), img1.double()
+    img0 = torch.clamp(img0, 0, 1)
+    img1 = torch.clamp(img1, 0, 1)
+    n, c, h, w = img0.shape
+    ph = ((h - 1) // 64 + 1) * 64
+    pw = ((w - 1) // 64 + 1) * 64
+    img0 = F.pad(img0, (0, pw - w, 0, ph - h))
+    img1 = F.pad(img1, (0, pw - w, 0, ph - h))
+    t = timestep.reshape(n, 1, 1, 1).to(img0.device).to(img0.dtype).repeat(1, 1, ph, pw)
+    hdt = None if dt is None else torch.float16
+    return img0, img1, t, (q16(img0, hdt), q16(img1, hdt)), dt
+
+
+def _head(sd: Dict[str, torch.Tensor], x: torch.Tensor, dt) -> torch.Tensor:
+    """Head (4.26) / Head_417 (4.17) with feat=False -- rife_arch.py:356-395: cnn0 3->c stride 2, cnn1, cnn2 c->c, each +
+    LeakyReLU(0.2), cnn3 ConvTranspose c->4|8.  With an operand: cnn0 on the CUDA cores with fp32 weights, cnn1..cnn3 with
+    weights rounded to T, every output stored in T."""
+    y = q16(F.leaky_relu(F.conv2d(x, *_wb(sd, "encode.cnn0.", dt, None), stride=2, padding=1), 0.2), dt)
+    y = q16(F.leaky_relu(F.conv2d(y, *_wb(sd, "encode.cnn1.", dt), padding=1), 0.2), dt)
+    y = q16(F.leaky_relu(F.conv2d(y, *_wb(sd, "encode.cnn2.", dt), padding=1), 0.2), dt)
+    return q16(F.conv_transpose2d(y, *_wb(sd, "encode.cnn3.", dt), stride=2, padding=1), dt)
+
+
+def _blend(img0, img1, flow, mask, w0, w1, dt):
+    """sigmoid blend of the last warps -- rife_arch.py:703-717.  With an operand the block inputs sampled the fp16 frames
+    (w0, w1) but the final warps read the fp32 ones."""
+    if dt is not None:
+        w0, w1 = warp(img0, flow[:, :2]), warp(img1, flow[:, 2:4])
+    m = torch.sigmoid(mask)
+    return w0 * m + w1 * (1 - m)
+
+
 def ifnet46_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torch.Tensor, timestep: torch.Tensor,
-                    scale_list: Sequence[float] = (8, 4, 2, 1), taps: Optional[dict] = None) -> torch.Tensor:
+                    scale_list: Sequence[float] = (8, 4, 2, 1), taps: Optional[dict] = None,
+                    operand: Optional[str] = None) -> torch.Tensor:
     """IFNet.forward restricted to arch 4.6, ensemble=False -- rife_arch.py:465-732.
 
     clamp + zero-pad right/bottom to x64 (:476-485), timestep plane (:491-494), block0 on
@@ -190,34 +287,27 @@ def ifnet46_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torch
     (SURVEY.md F7), so they are not parameters here.
     NCHW fp32 in, NCHW fp32 out; ``timestep`` is [B,1,1,1].
     """
-    img0 = torch.clamp(img0, 0, 1)
-    img1 = torch.clamp(img1, 0, 1)
-    n, c, h, w = img0.shape
-    ph = ((h - 1) // 64 + 1) * 64
-    pw = ((w - 1) // 64 + 1) * 64
-    img0 = F.pad(img0, (0, pw - w, 0, ph - h))
-    img1 = F.pad(img1, (0, pw - w, 0, ph - h))
-    t = timestep.reshape(n, 1, 1, 1).to(img0.dtype).repeat(1, 1, ph, pw)
-    w0, w1, flow, mask = img0, img1, None, None
+    h, w = img0.shape[2], img0.shape[3]
+    img0, img1, t, (h0, h1), dt = _prep(img0, img1, timestep, operand)
+    w0, w1, flow, mask = h0, h1, None, None
     for i in range(4):
         if flow is None:
-            flow, mask = ifblock(sd, i, torch.cat((img0, img1, t), 1), None, scale_list[i], taps)
+            flow, mask = ifblock(sd, i, torch.cat((h0, h1, t), 1), None, scale_list[i], taps, operand)
         else:
-            f0, m0 = ifblock(sd, i, torch.cat((w0, w1, t, mask), 1), flow, scale_list[i], taps)
+            f0, m0 = ifblock(sd, i, torch.cat((w0, w1, t, mask), 1), flow, scale_list[i], taps, operand)
             flow = flow + f0
             mask = mask + m0
         if taps is not None:
             taps[f"flow{i}"] = flow
             taps[f"mask{i}"] = mask
-        w0 = warp(img0, flow[:, :2])
-        w1 = warp(img1, flow[:, 2:4])
-    m = torch.sigmoid(mask)
-    merged = w0 * m + w1 * (1 - m)
-    return merged[:, :, :h, :w]
+        w0 = warp(h0, flow[:, :2])
+        w1 = warp(h1, flow[:, 2:4])
+    return _blend(img0, img1, flow, mask, w0, w1, dt)[:, :, :h, :w]
 
 
 def ifnet47_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torch.Tensor, timestep: torch.Tensor,
-                    scale_list: Sequence[float] = (8, 4, 2, 1), taps: Optional[dict] = None) -> torch.Tensor:
+                    scale_list: Sequence[float] = (8, 4, 2, 1), taps: Optional[dict] = None,
+                    operand: Optional[str] = None) -> torch.Tensor:
     """IFNet.forward restricted to arch 4.7 (rife47.pth / rife49.pth) and 4.17 (rife417.pth, same forward with the
     Head_417 encoder and 8 feature channels per frame), ensemble=False -- rife_arch.py:465-732.
 
@@ -225,48 +315,40 @@ def ifnet47_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torch
     concatenated to block 0's input (:543-548) and, warped with the current flow, to the later blocks' inputs
     (:629-645); `flow = flow + fd` but `mask = m0` is REPLACED, not accumulated (:646, :698-699); the final blend
     uses sigmoid of that last mask (:721-723)."""
-    img0 = torch.clamp(img0, 0, 1)
-    img1 = torch.clamp(img1, 0, 1)
-    n, c, h, w = img0.shape
-    ph = ((h - 1) // 64 + 1) * 64
-    pw = ((w - 1) // 64 + 1) * 64
-    img0 = F.pad(img0, (0, pw - w, 0, ph - h))
-    img1 = F.pad(img1, (0, pw - w, 0, ph - h))
-    t = timestep.reshape(n, 1, 1, 1).to(img0.dtype).repeat(1, 1, ph, pw)
+    h, w = img0.shape[2], img0.shape[3]
+    img0, img1, t, (h0, h1), dt = _prep(img0, img1, timestep, operand)
 
     def encode(x):
         if "encode.cnn0.weight" in sd:  # arch 4.17, Head_417.forward -- rife_arch.py:365-375 (feat=False)
-            y = F.leaky_relu(F.conv2d(x, sd["encode.cnn0.weight"], sd["encode.cnn0.bias"], stride=2, padding=1), 0.2)
-            y = F.leaky_relu(F.conv2d(y, sd["encode.cnn1.weight"], sd["encode.cnn1.bias"], padding=1), 0.2)
-            y = F.leaky_relu(F.conv2d(y, sd["encode.cnn2.weight"], sd["encode.cnn2.bias"], padding=1), 0.2)
-            return F.conv_transpose2d(y, sd["encode.cnn3.weight"], sd["encode.cnn3.bias"], stride=2, padding=1)
-        y = F.conv2d(x, sd["encode.0.weight"], sd["encode.0.bias"], stride=2, padding=1)
-        return F.conv_transpose2d(y, sd["encode.1.weight"], sd["encode.1.bias"], stride=2, padding=1)
+            return _head(sd, x, dt)
+        # arch 4.7: both layers on the CUDA cores with fp32 weights, the features stored as fp16 whatever T is
+        y = F.conv2d(x, *_wb(sd, "encode.0.", dt, None), stride=2, padding=1)
+        y = F.conv_transpose2d(y, *_wb(sd, "encode.1.", dt, None), stride=2, padding=1)
+        return q16(y, None if dt is None else torch.float16)
 
     f0, f1 = encode(img0), encode(img1)
     if taps is not None:
         taps["f0"], taps["f1"] = f0, f1
-    w0, w1, flow, mask = img0, img1, None, None
+    w0, w1, flow, mask = h0, h1, None, None
     for i in range(4):
         if flow is None:
-            flow, mask = ifblock(sd, i, torch.cat((img0, img1, f0, f1, t), 1), None, scale_list[i], taps)
+            flow, mask = ifblock(sd, i, torch.cat((h0, h1, f0, f1, t), 1), None, scale_list[i], taps, operand)
         else:
             fd, m0 = ifblock(sd, i, torch.cat((w0, w1, warp(f0, flow[:, :2]), warp(f1, flow[:, 2:4]), t, mask), 1),
-                             flow, scale_list[i], taps)
+                             flow, scale_list[i], taps, operand)
             flow = flow + fd
             mask = m0
         if taps is not None:
             taps[f"flow{i}"] = flow
             taps[f"mask{i}"] = mask
-        w0 = warp(img0, flow[:, :2])
-        w1 = warp(img1, flow[:, 2:4])
-    m = torch.sigmoid(mask)
-    merged = w0 * m + w1 * (1 - m)
-    return merged[:, :, :h, :w]
+        w0 = warp(h0, flow[:, :2])
+        w1 = warp(h1, flow[:, 2:4])
+    return _blend(img0, img1, flow, mask, w0, w1, dt)[:, :, :h, :w]
 
 
 def ifnet426_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torch.Tensor, timestep: torch.Tensor,
-                     scale_list: Sequence[float] = (16, 8, 4, 2, 1), taps: Optional[dict] = None) -> torch.Tensor:
+                     scale_list: Sequence[float] = (16, 8, 4, 2, 1), taps: Optional[dict] = None,
+                     operand: Optional[str] = None) -> torch.Tensor:
     """IFNet.forward restricted to arch 4.26 (rife426.pth; the node forces ensemble=False, rife/__init__.py:123-125)
     -- rife_arch.py:465-732.
 
@@ -275,48 +357,34 @@ def ifnet426_forward(sd: Dict[str, torch.Tensor], img0: torch.Tensor, img1: torc
     (:521-526); block i > 0 sees cat(warped0, warped1, warp(f0), warp(f1), t, mask, feat) + flow, where `feat` is the
     previous block's 8 extra lastconv channels up-scaled to full resolution (:563-587); `flow += fd`, `mask = m0`
     REPLACED (:586-587); blend with sigmoid of the last mask (:707-711)."""
-    img0 = torch.clamp(img0, 0, 1)
-    img1 = torch.clamp(img1, 0, 1)
-    n, c, h, w = img0.shape
-    ph = ((h - 1) // 64 + 1) * 64
-    pw = ((w - 1) // 64 + 1) * 64
-    img0 = F.pad(img0, (0, pw - w, 0, ph - h))
-    img1 = F.pad(img1, (0, pw - w, 0, ph - h))
-    t = timestep.reshape(n, 1, 1, 1).to(img0.dtype).repeat(1, 1, ph, pw)
+    h, w = img0.shape[2], img0.shape[3]
+    img0, img1, t, (h0, h1), dt = _prep(img0, img1, timestep, operand)
 
-    def encode(x):  # Head.forward, feat=False -- rife_arch.py:387-395
-        y = F.leaky_relu(F.conv2d(x, sd["encode.cnn0.weight"], sd["encode.cnn0.bias"], stride=2, padding=1), 0.2)
-        y = F.leaky_relu(F.conv2d(y, sd["encode.cnn1.weight"], sd["encode.cnn1.bias"], padding=1), 0.2)
-        y = F.leaky_relu(F.conv2d(y, sd["encode.cnn2.weight"], sd["encode.cnn2.bias"], padding=1), 0.2)
-        return F.conv_transpose2d(y, sd["encode.cnn3.weight"], sd["encode.cnn3.bias"], stride=2, padding=1)
-
-    f0, f1 = encode(img0), encode(img1)
+    f0, f1 = _head(sd, img0, dt), _head(sd, img1, dt)  # Head.forward, feat=False -- rife_arch.py:387-395
     if taps is not None:
         taps["f0"], taps["f1"] = f0, f1
-    w0, w1, flow, mask, feat = img0, img1, None, None, None
+    w0, w1, flow, mask, feat = h0, h1, None, None, None
     for i in range(5):
         if flow is None:
-            flow, mask, feat = ifblock(sd, i, torch.cat((img0, img1, f0, f1, t), 1), None, scale_list[i], taps)
+            flow, mask, feat = ifblock(sd, i, torch.cat((h0, h1, f0, f1, t), 1), None, scale_list[i], taps, operand)
         else:
             x = torch.cat((w0, w1, warp(f0, flow[:, :2]), warp(f1, flow[:, 2:4]), t, mask, feat), 1)
-            fd, m0, feat = ifblock(sd, i, x, flow, scale_list[i], taps)
+            fd, m0, feat = ifblock(sd, i, x, flow, scale_list[i], taps, operand)
             flow = flow + fd
             mask = m0
         if taps is not None:
             taps[f"flow{i}"] = flow
             taps[f"mask{i}"] = mask
-        w0 = warp(img0, flow[:, :2])
-        w1 = warp(img1, flow[:, 2:4])
-    m = torch.sigmoid(mask)
-    merged = w0 * m + w1 * (1 - m)
-    return merged[:, :, :h, :w]
+        w0 = warp(h0, flow[:, :2])
+        w1 = warp(h1, flow[:, 2:4])
+    return _blend(img0, img1, flow, mask, w0, w1, dt)[:, :, :h, :w]
 
 
-def ifnet_forward(arch: str, sd, img0, img1, timestep, scale_list=None, taps=None):
+def ifnet_forward(arch: str, sd, img0, img1, timestep, scale_list=None, taps=None, operand=None):
     if scale_list is None:
         scale_list = SCALE_LIST[arch]
     fn = ifnet46_forward if arch == "4.6" else ifnet426_forward if arch == "4.26" else ifnet47_forward
-    return fn(sd, img0, img1, timestep, scale_list, taps)
+    return fn(sd, img0, img1, timestep, scale_list, taps, operand)
 
 
 # --------------------------------------------------------------------------------------

@@ -18,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from make_golden import cases, make_inputs  # noqa: E402
 from oracle import rife46 as O  # noqa: E402
+import rife16_util as U  # noqa: E402
 
 CUDA_INC = "/usr/local/cuda/include"
 
@@ -41,6 +42,51 @@ def _engine_names(arch):
     ge.load_package()
     from cfi_b200.engine import ARCH_CODE, state_dict_names
     return state_dict_names(arch), ARCH_CODE[arch]
+
+
+def _run(emu, arch, sd, fr, ts, sf, operand):
+    """One emulated vfi_rife46_forward of the tasks (0, 1, ts[i]): (frames [B,h,w,3], flow [B,Hp,Wp,4], mask [B,Hp,Wp])."""
+    names, code = _engine_names(arch)
+    hold = [sd[n].contiguous().float() for n in names]
+    ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+    numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+    ctx = C.c_void_p()
+    assert emu.vfi_create(0, C.byref(ctx)) == 0, emu.vfi_last_error()
+    assert emu.vfi_rife_load(ctx, code, ptrs, numel, len(hold), 0 if operand == "float16" else 1) == 0, emu.vfi_last_error()
+    fr = fr.contiguous()
+    n, h, w, c = fr.shape
+    b = len(ts)
+    t = np.asarray(ts, np.float32)
+    f0, f1 = np.zeros(b, np.int32), np.ones(b, np.int32)
+    vp = lambda x: x.ctypes.data_as(C.c_void_p)   # noqa: E731
+    out = torch.zeros(b, h, w, 3)
+    assert emu.vfi_rife46_forward(ctx, C.c_void_p(fr.data_ptr()), n, h, w, c, vp(f0), vp(f1), vp(t), b, C.c_float(sf),
+                                  C.c_void_p(out.data_ptr()), None) == 0, emu.vfi_last_error()
+    hp, wp = C.c_int(), C.c_int()
+    assert emu.vfi_rife46_debug_state(ctx, None, None, b, C.byref(hp), C.byref(wp)) == 0, emu.vfi_last_error()
+    flow, mask = torch.zeros(b, hp.value, wp.value, 4), torch.zeros(b, hp.value, wp.value)
+    assert emu.vfi_rife46_debug_state(ctx, C.c_void_p(flow.data_ptr()), C.c_void_p(mask.data_ptr()), b, C.byref(hp),
+                                      C.byref(wp)) == 0, emu.vfi_last_error()
+    assert emu.vfi_destroy(ctx) == 0
+    return out, flow, mask
+
+
+def _check_faithful(emu, label, arch, sd, fr, ts, sf, operand):
+    """The emulated path against the 16-bit-faithful float64 oracle, per pixel (tests/rife16_util.py)."""
+    got = _run(emu, arch, sd, fr, ts, sf, operand)
+    want = U.oracle(arch, sd, fr, [0] * len(ts), [1] * len(ts), ts, sf, operand)
+    lines, fails = U.compare(f"{label} {operand}", got, want, fr.shape[1], fr.shape[2], U.tol(label, operand))
+    print("\n".join(lines))
+    assert not fails, "\n".join(fails)
+
+
+@pytest.mark.parametrize("operand", ["float16", "bfloat16"])
+@pytest.mark.parametrize("arch,sf,h,w", [pytest.param(*c, id=U.case_id(*c)) for c in U.cases()])
+def test_rife_whole_path_on_host_matches_faithful_oracle(emu, arch, sf, h, w, operand):
+    """Odd sizes, a thin strip, t near 0 and 1 and every scale_factor: frames, full-resolution flow and mask of the
+    emulated library against the 16-bit-faithful oracle, over the whole plane and over its border band."""
+    sd, fr = U.inputs(arch, h, w)
+    _check_faithful(emu, U.case_id(arch, sf, h, w), arch, sd, fr, list(U.TIMESTEPS), sf, operand)
 
 
 @pytest.mark.parametrize("name", ["ifnet_64x64_gain4", "ifnet47_64x128_gain3", "ifnet417_64x128_gain3",
@@ -78,6 +124,7 @@ def test_rife_whole_path_on_host_matches_reference(emu, name):
     psnr = 99.0 if mse == 0 else 10 * math.log10(1.0 / mse)
     print(f"host emulation of the whole RIFE {arch} path ({name}): {launches} launches, PSNR {psnr:.2f} dB")
     assert psnr >= 60.0, psnr
+    _check_faithful(emu, name, arch, sd, fr, list(cfg["ts"]), cfg.get("scale_factor", 1.0), "float16")
 
 
 def test_rife_bf16_operands_on_host(emu):
@@ -106,6 +153,18 @@ def test_rife_bf16_operands_on_host(emu):
     psnr = 10 * math.log10(1.0 / mse)
     print(f"host emulation, bf16 operands ({name}): PSNR {psnr:.2f} dB")
     assert psnr >= 50.0, psnr
+
+
+@pytest.mark.parametrize("name", ["ifnet_64x64_gain4", "ifnet47_64x128_gain3", "ifnet417_64x128_gain3",
+                                  "ifnet426_128x128_gain3", "ifnet_64x64_sf2", "ifnet_64x64_sf4", "ifnet47_64x64_sf2",
+                                  "ifnet47_64x64_sf4", "ifnet417_64x64_sf2", "ifnet426_64x64_sf2",
+                                  "ifnet426_64x64_sf4", "ifnet_40x100_sf2", "ifnet426_40x100_sf4"])
+def test_rife_bf16_golden_cases_on_host_match_faithful_oracle(emu, name):
+    """The golden cases with bf16 operands against the 16-bit-faithful oracle, per pixel."""
+    cfg = cases()[name]
+    arch = cfg.get("arch", "4.6")
+    sd = O.synthetic_state_dict(cfg["seed"], cfg["gain"], arch=arch)
+    _check_faithful(emu, name, arch, sd, make_inputs(cfg), list(cfg["ts"]), cfg.get("scale_factor", 1.0), "bfloat16")
 
 
 def test_rife_host_pipeline_on_host_matches_reference_node(emu):
