@@ -60,7 +60,7 @@ def lib():
     L.vfi_rife46_debug_layer.argtypes = [vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]
     L.vfi_rife46_debug_state.argtypes = [vp, vp, vp, i32, C.POINTER(i32), C.POINTER(i32)]
     L.vfi_rife46_layer_plan.argtypes = [vp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
-                                        C.POINTER(i32), C.POINTER(i64), C.POINTER(i32)]
+                                        C.POINTER(i32), C.POINTER(i64), C.POINTER(i32), C.POINTER(i32)]
     L.vfi_sync.argtypes = [vp]
     L.vfi_rife_profile.argtypes = [vp, i32]
     L.vfi_host_copy_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32]

@@ -258,10 +258,11 @@ void set_taps_3x3(TapConvLayer& L, int ch, bool ring) {
     }
 }
 
-// Wide, deep layers (c = 128, 192): with the whole window staged per tile the resident weight slice leaves room for
-// only n_cta = 16 output channels, and every wgmma reads its whole 64-row A block from shared memory whatever its N, so
-// narrow CTAs re-read the window once per split.  The ring pipeline stages one 64-channel k-block at a time, which
-// frees shared memory for n_cta = 32 (c = 192) / 64 (c = 128).  VFI_RING=0 disables it (A/B runs).
+// Wide, deep layers (c = 128, 192; the ResConvs stream their weights instead): with the whole window staged
+// per tile the resident weight slice leaves room for only n_cta = 16 output channels, and every wgmma reads its whole
+// 64-row A block from shared memory whatever its N, so narrow CTAs re-read the window once per split.  The ring
+// pipeline stages one 64-channel k-block at a time, which frees shared memory for n_cta = 32 (c = 192) / 64 (c = 128).
+// VFI_RING=0 disables it (A/B runs).
 bool want_ring(int ch) {
   static const bool on = [] {
     const char* e = std::getenv("VFI_RING");
@@ -278,12 +279,31 @@ int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const 
   L.ktotal16 = 9 * (ch / 16);
   L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
   L.epi_mode = EPI_RESCONV;
-  const bool ring = want_ring(ch);
-  set_taps_3x3(L, ch, ring);
-  choose_split(L, {1, 2, 3, 4, 6, 8, 12}, ring ? 2 : 3);
+  int real_taps = 9;
+  if (ch >= 96) {
+    // streamed weights (tapconv.cu): all channels per CTA up to the wgmma's N = 128, else two halves of 96.  The taps
+    // keep the K order of the resident-weight plans: k-block-major (the ring's) at c = 128 / 192, tap-major at c = 96.
+    set_taps_3x3(L, ch, ch % 64 == 0);
+    real_taps = L.ntaps;
+    L.ring = 0;
+    L.wstream = 1;
+    L.nsplit = ch > 128 ? 2 : 1;
+    L.n_cta = ch / L.nsplit;
+    if (L.ktotal16 & 3) {  // c = 96: 54 K=16 steps; two more with zero weights fill the last four-step weight slot
+      TapEntry& t = L.taps[L.ntaps++];
+      t.dy = 0; t.dx = 0; t.chunk0 = 0;
+      t.nk16 = (int16_t)(4 - (L.ktotal16 & 3));
+      L.ktotal16 += t.nk16;
+    }
+  } else {
+    const bool ring = want_ring(ch);
+    set_taps_3x3(L, ch, ring);
+    choose_split(L, {1, 2, 3, 4, 6, 8, 12}, ring ? 2 : 3);
+  }
   // (conv(x) + b) * beta + x  ==  conv_{w*beta}(x) + b*beta + x : beta is folded into the packed weights (one 16-bit
   // rounding of w*beta instead of w) so the epilogue is a pure add
   auto wf = [&](int e, int ci, int n) -> float {  // e = kb * 9 + tap (kb = 0 unless ring), ci relative to the k-block
+    if (e >= real_taps) return 0.f;
     const int tap = e % 9, cin = (e / 9) * 64 + ci;
     return w[(((size_t)n * ch + cin) * 3 + tap / 3) * 3 + tap % 3] * beta[n];
   };
@@ -1437,7 +1457,7 @@ int vfi_rife46_debug_state(vfi_ctx* c, float* flow4_out, float* mask_out, int ba
 }
 
 int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
-                          int64_t* macs_per_cell, int* cmajor) {
+                          int64_t* macs_per_cell, int* cmajor, int* wstream) {
   if (!c || block < 0 || layer < 0) return fail(VFI_E_INVALID, "bad argument");
   if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
   if (block >= num_blocks(c->arch) || layer > 11 || (layer == 11 && (c->arch != 426 || block + 1 >= num_blocks(c->arch))))
@@ -1449,8 +1469,10 @@ int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_
   if (n_cta) *n_cta = L.n_cta;
   if (nsplit) *nsplit = L.nsplit;
   if (smem_bytes) *smem_bytes = (int)p.smem_bytes;
-  if (macs_per_cell) *macs_per_cell = (int64_t)L.ktotal16 * 16 * L.n_total;
+  // (a streamed c = 96 ResConv issues two more K=16 steps with zero weights than its 9 x 96 products per output)
+  if (macs_per_cell) *macs_per_cell = (int64_t)(L.epi_mode == EPI_RESCONV ? 9 * L.cin : L.ktotal16 * 16) * L.n_total;
   if (cmajor) *cmajor = p.cmajor;
+  if (wstream) *wstream = p.wstream;
   return VFI_OK;
 }
 

@@ -26,7 +26,18 @@
 // in the same K order into fp32: the outputs are bit-identical to the cell-major form (DESIGN.md section 5 has the
 // measured gain).
 //
-// Warp roles (288 threads, 1 CTA/SM, persistent over tiles):
+// Streamed weights (p.wstream, template WS: the wide ResConvs, c = 96 / 128 / 192).  A resident weight slice of such a
+// layer leaves room for only 48 - 64 output channels per CTA, so every tile's window was read from L2 and shared memory
+// once per output-channel split (2 - 4 times), and the narrow wgmma N left the tensor cores waiting on shared memory
+// (an SS wgmma reads its 2 KB A block whatever its N).  Here the window of a tile is staged once with all its k-blocks
+// and held until the epilogue, and the weights stream through a ring of slots of four K=16 steps each (the packed
+// [K16 / 4][n_cta][128 B] rows, one bulk copy per slot) fed by a second producer warp: n_cta = 96 / 128 / 96 output
+// channels per CTA.  Both MMA warpgroups take a tile each and consume every slot in step, so one weight fill from L2
+// feeds 256 cells.  The K=16 steps keep the order of the layer's tap list (k-block-major at c = 128 / 192 as the ring
+// plan issued them, tap-major at c = 96, whose two extra zero-weight steps only complete the last slot): every output
+// is the same fp32 sum in the same order as with resident weights.
+//
+// Warp roles (288 threads, 1 CTA/SM, persistent over tiles; WS: 320):
 //   warpgroups 0, 1 : MMA + epilogue.  Warpgroup w takes the CTA's tiles w, w + 2, ... and keeps the whole tile's
 //                     accumulators (2 x 64 rows x n_cta columns, fp32) in registers, so one warpgroup's epilogue
 //                     overlaps the other's MMAs: +shift (held in registers for the launch), +residual (non-ring
@@ -35,6 +46,8 @@
 //                     per-warpgroup staging tile and leave as TMA tensor stores (one thread, clipped at the image
 //                     border); lastconv writes whole float4 flow texels, the space-to-depth forms direct stores.
 //   warp 8          : one elected lane: weight bulk copy, then one 4-D TMA tensor copy per k-block and tile
+//   warp 9 (WS)     : one elected lane: one bulk copy per weight slot, the whole weight stream once per pair of tiles
+#include <algorithm>
 #include <cstdlib>
 #include <type_traits>
 
@@ -46,13 +59,17 @@ namespace vfi {
 namespace {
 
 constexpr int kMaxStages = 6;   // window stages or ring slots
+constexpr int kMaxWSlots = 8;   // streamed weight slots
 struct Ctrl {
   uint64_t w_full;
   uint64_t a_full[kMaxStages][2];  // [stage][consuming warpgroup]
   uint64_t a_empty[kMaxStages];
+  uint64_t ws_full[kMaxWSlots];    // WS: weight slot filled (bulk-copy bytes)
+  uint64_t ws_empty[kMaxWSlots];   // WS: every warp of both MMA warpgroups has read the slot
 };
-constexpr uint32_t kCtrlBytes = 256;
-constexpr int kMmaGroups = 2, kTmaWarp = 8, kThreads = 128 * kMmaGroups + 32;
+constexpr uint32_t kCtrlBytes = 512;
+constexpr int kMmaGroups = 2, kTmaWarp = 8, kWeightWarp = 9, kThreads = 128 * kMmaGroups + 32;
+constexpr int kThreadsWS = kThreads + 32;
 static_assert(sizeof(Ctrl) <= kCtrlBytes, "control block");
 constexpr int kCmRuns = 9, kCmRunLen = 4;  // channel-major MMA issue: 9 taps x 4 K=16 steps (64 input channels)
 
@@ -152,9 +169,29 @@ __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc
   }
 }
 
-template <typename T, bool RING, bool LAST, int N, bool CM>
-__global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_constant__ TapConvParams p) {
+// WS: the MMAs of weight slot `grp` (K=16 steps 4 grp .. 4 grp + 3; tapconv_plan admits K16 % 4 == 0 only) for both
+// 64-row halves of the tile.  p.mma[j] is step j's window descriptor; its weights start 32 B * (j % 4) into the slot.
+// Straight-line: a conditional exit between the MMAs makes ptxas serialize every wgmma of the kernel (C7520).
+template <int N, typename T>
+__device__ __forceinline__ void issue_wslot(const TapConvParams& p, float (&acc)[2][N / 2], uint32_t a_base,
+                                            uint32_t b_base, int grp) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int j = 4 * grp + i;
+    const uint4 d = p.mma[j];
+    const uint32_t half_off = 8u * (d.y & 0x3fffu);
+    const uint64_t b64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b_base + 2u * i);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      wgmma_ss<N, T>(acc[h], ((uint64_t)d.y << 32) | (uint64_t)(a_base + d.x + (uint32_t)h * half_off), b64,
+                     j ? 1u : 0u);
+  }
+}
+
+template <typename T, bool RING, bool LAST, int N, bool CM, bool WS>
+__global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(const __grid_constant__ TapConvParams p) {
   static_assert(!CM || (N == 64 && !RING && !LAST), "channel-major: 64 output channels, staged window, 16-bit output");
+  static_assert(!WS || (!CM && !RING && !LAST), "streamed weights: cells on M, staged window, 16-bit output");
   extern __shared__ __align__(1024) uint8_t smem[];
   // Programmatic dependent launch (launch_tapconv sets the attribute): the next kernel in the stream may start its
   // CTAs as soon as every CTA of this grid has passed this point, i.e. while our last tiles are still running - they do
@@ -178,6 +215,8 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   const uint32_t bar_w = smem_base + offsetof(Ctrl, w_full);
   const uint32_t bar_afull = smem_base + offsetof(Ctrl, a_full);
   const uint32_t bar_aempty = smem_base + offsetof(Ctrl, a_empty);
+  const uint32_t bar_wsfull = smem_base + offsetof(Ctrl, ws_full);
+  const uint32_t bar_wsempty = smem_base + offsetof(Ctrl, ws_empty);
   const uint32_t a_smem = smem_base + p.off_a;
   const uint32_t w_smem = smem_base + p.off_w;
   const bool has_tail = (p.cin & 63) != 0;  // last k-block is 32 channels wide
@@ -189,17 +228,43 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
       mbar_init(bar_afull + 16 * s + 8, 1);
       mbar_init(bar_aempty + 8 * s, 4);      // the four warps of the consuming warpgroup
     }
+    if (WS)
+      for (int s = 0; s < p.w_slots; ++s) {
+        mbar_init(bar_wsfull + 8 * s, 1);
+        mbar_init(bar_wsempty + 8 * s, 4 * kMmaGroups);
+      }
     mbar_fence_init();
   }
   __syncthreads();
 
+  if (WS && warp == kWeightWarp) {
+    // ======================================================= weight producer: the slots of every pass of two tiles
+    if (lane == 0) {
+      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_bytes;
+      uint32_t slot = 0, ph = 0;
+      for (int q = 0; q < (my_tiles + 1) / 2; ++q)
+        for (int grp = 0; grp < p.w_groups; ++grp) {
+          mbar_wait(bar_wsempty + 8 * slot, ph ^ 1u);
+          mbar_arrive_expect_tx(bar_wsfull + 8 * slot, p.w_slot_bytes);
+          bulk_g2s(w_smem + slot * p.w_slot_bytes, wsrc + (size_t)grp * p.w_slot_bytes, p.w_slot_bytes,
+                   bar_wsfull + 8 * slot);
+          if (++slot == (uint32_t)p.w_slots) {
+            slot = 0;
+            ph ^= 1u;
+          }
+        }
+    }
+    return;
+  }
   if (warp == kTmaWarp) {
     // ======================================================= TMA producer (one thread feeds the whole pipeline)
     if (lane == 0) {
-      mbar_arrive_expect_tx(bar_w, p.w_bytes);
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_bytes;
-      for (uint32_t off = 0; off < p.w_bytes; off += 32768u)
-        bulk_g2s(w_smem + off, wsrc + off, min(32768u, p.w_bytes - off), bar_w);
+      if (!WS) {
+        mbar_arrive_expect_tx(bar_w, p.w_bytes);
+        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w) + (size_t)split * p.w_bytes;
+        for (uint32_t off = 0; off < p.w_bytes; off += 32768u)
+          bulk_g2s(w_smem + off, wsrc + off, min(32768u, p.w_bytes - off), bar_w);
+      }
       // weights do not depend on the previous kernel; its output (our input tensor) does
       asm volatile("griddepcontrol.wait;" ::: "memory");
       TileIter it(p, first, tstep);
@@ -245,19 +310,19 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   const int px = lane >> 2;             // tile column of this thread's accumulator rows
   const int c2 = 2 * (lane & 3);        // first of this thread's two columns in every 8-column block
   // the CTA's output-channel slice is fixed: its shift values stay in registers for the whole launch (channel-major:
-  // this thread's two channels 16 wq + lane / 4, +8)
-  float2 sh[CM ? 1 : N / 8];
+  // this thread's two channels 16 wq + lane / 4, +8; WS: read per tile, the registers hold the N = 128 accumulators)
+  float2 sh[(CM || WS) ? 1 : N / 8];
   if constexpr (CM) {
     const int ch = n0 + 16 * wq + (lane >> 2);
     sh[0] = make_float2(__ldg(p.shift + ch), __ldg(p.shift + ch + 8));
-  } else {
+  } else if constexpr (!WS) {
 #pragma unroll
     for (int j = 0; j < N / 8; ++j) sh[j] = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
   }
   // the previous kernel may still be reading the buffer we store to (ping-pong) and ring ResConv layers read the
   // residual from global memory: every storing / loading thread orders itself after the previous grid
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  mbar_wait(bar_w, 0);
+  if (!WS) mbar_wait(bar_w, 0);
   const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);  // LBO(=1) | start address, 16-byte units
   const uint32_t b_lo0 = (1u << 16) | (w_smem >> 4);
   const uint32_t per_tile = RING ? (uint32_t)p.nkb : 1u;  // stages / slots one tile consumes
@@ -282,10 +347,39 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
   const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for the warpgroup's bulk groups
   const uint32_t out_smem = smem_base + p.off_out + (uint32_t)g * p.out_stage_bytes;
   float acc[2][N / 2];
+  uint32_t wslot = 0, wph = 0;  // WS: next weight slot and the parity of its "full" barrier
+  const uint32_t w_slot_units = p.w_slot_bytes >> 4;
+  auto next_wslot = [&]() {
+    if (++wslot == (uint32_t)p.w_slots) {
+      wslot = 0;
+      wph ^= 1u;
+    }
+  };
 
   TileIter it(p, first + g * tstep, kMmaGroups * tstep);
   for (int k = g; k < my_tiles; k += kMmaGroups, it.next()) {
-    if (RING) {
+    if (WS) {
+      wait_full();
+      const uint32_t a_base = a_lo0 + stage * stage_units;
+      uint32_t prev = 0;
+      for (int grp = 0; grp < p.w_groups; ++grp) {
+        mbar_wait(bar_wsfull + 8 * wslot, wph);
+        wgmma_fence();
+        issue_wslot<N, T>(p, acc, a_base, b_lo0 + wslot * w_slot_units, grp);
+        wgmma_commit();
+        if (grp > 0) {  // the previous slot's MMAs have read it
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_wsempty + 8 * prev);
+        }
+        prev = wslot;
+        next_wslot();
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_wsempty + 8 * prev);
+      if (!residual && lane == 0) mbar_arrive(bar_aempty + 8 * stage);
+    } else if (RING) {
       uint32_t prev = 0;
       for (int kb = 0; kb < p.nkb; ++kb) {
         wait_full();
@@ -337,10 +431,15 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
-          acc[h][4 * j] += sh[j].x;
-          acc[h][4 * j + 1] += sh[j].y;
-          acc[h][4 * j + 2] += sh[j].x;
-          acc[h][4 * j + 3] += sh[j].y;
+          float2 s;
+          if constexpr (WS)
+            s = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
+          else
+            s = sh[j];
+          acc[h][4 * j] += s.x;
+          acc[h][4 * j + 1] += s.y;
+          acc[h][4 * j + 2] += s.x;
+          acc[h][4 * j + 3] += s.y;
         }
     }
     if (residual && !RING) {
@@ -527,6 +626,14 @@ __global__ void __launch_bounds__(kThreads, 1) tapconv_kernel(const __grid_const
         }
       }
   }
+  if (WS && (my_tiles & 1) && g == 1) {  // the last pass has no tile for warpgroup 1: it still releases every slot
+    for (int grp = 0; grp < p.w_groups; ++grp) {
+      mbar_wait(bar_wsfull + 8 * wslot, wph);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_wsempty + 8 * wslot);
+      next_wslot();
+    }
+  }
   if (tma_out && leader) bulk_wait<0>();  // the CTA's last stores have landed before it exits
 }
 
@@ -659,11 +766,14 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   // input window: one 1024-aligned region per k-block (64 channels = 128-byte rows; 32-channel tail = 64-byte rows)
   p.nkb = (L.cin + 63) / 64;
   p.ring = L.ring;
+  p.wstream = L.wstream;
   if (L.ktotal16 > kMaxK16) return 0;
   // n_cta = the wgmma N: whole 8-row swizzle atoms of B, and a multiple of 16 with an instantiated kernel (<= 96: two
   // 64-row accumulators of n_cta fp32 columns per thread)
-  if (p.nkb > kMaxKBlocks || L.n_cta > 96 || (L.n_cta & 15) || L.n_cta < 16) return 0;
+  // (streamed weights, whose shift is read per tile instead: up to 128)
+  if (p.nkb > kMaxKBlocks || L.n_cta > (L.wstream ? 128 : 96) || (L.n_cta & 15) || L.n_cta < 16) return 0;
   if (L.ring && ((L.cin & 63) || L.ntaps != 9 * p.nkb || L.ktotal16 != 36 * p.nkb)) return 0;
+  if (L.wstream && (L.ring || L.epi_mode == EPI_LASTCONV || L.out_s2d != 0 || (L.ktotal16 & 3))) return 0;
   uint32_t off = 0;
   p.tx_bytes = 0;
   if (L.ring) {
@@ -703,9 +813,11 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
                              b_off >> 4, 0u);
       }
     // group the steps into runs of run_len = 4, 2 or 1 whose descriptors advance by 32 B (2 units) per step
+    // (streamed weights: one entry per step, issue_wslot)
     const int nsteps = L.ring ? 36 : L.ktotal16;  // ring: the first k-block's entries serve every slot
     int run_len = 1;
     for (int len : {4, 2}) {
+      if (L.wstream) break;
       bool ok = (nsteps % len) == 0;
       for (int r = 0; ok && r < nsteps; r += len)
         for (int i = 1; i < len; ++i)
@@ -737,6 +849,32 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
     return 0;
   };
   int stages = 0;
+  p.w_groups = (L.ktotal16 + 3) / 4;
+  p.w_slot_bytes = (uint32_t)L.n_cta * 128u;
+  p.w_slots = 0;
+  if (L.wstream) {
+    // the weight region holds w_slots slots of four K=16 steps.  Preference: the staged stores (both warpgroups run
+    // their epilogues at once, the tensor cores idle meanwhile), then 4 window stages (the next pass's windows load
+    // during this one) down to the 2 the two tiles of a pass need, each with at least 3 weight slots in flight
+    constexpr int kMinWSlots = 3;
+    for (uint32_t out_stage : {(uint32_t)(kTileH * kTileW) * L.n_cta * 2u, 0u})
+      for (int s = 4; s >= 2 && p.w_slots == 0; --s) {
+        const uint32_t fixed = align_up(kCtrlBytes, 1024) + kMmaGroups * out_stage + (uint32_t)s * p.stage_bytes;
+        if (fixed >= (uint32_t)kSmemLimit) continue;
+        const int slots = std::min<int>({(int)(((uint32_t)kSmemLimit - fixed) / p.w_slot_bytes), kMaxWSlots, p.w_groups});
+        if (slots < std::min(kMinWSlots, p.w_groups)) continue;
+        p.w_slots = slots;
+        p.w_bytes = (uint32_t)slots * p.w_slot_bytes;  // (resident size for fit(); restored below)
+        stages = fit(out_stage);
+        p.w_bytes = (uint32_t)p.w_groups * p.w_slot_bytes;
+        break;
+      }
+    if (p.w_slots == 0) return 0;
+    p.stages = stages;
+    p.smem_bytes = p.off_a + (uint32_t)stages * p.stage_bytes;
+    p.cmajor = 0;
+    return stages;
+  }
   if (L.epi_mode != EPI_LASTCONV && L.out_s2d == 0) stages = fit((uint32_t)(kTileH * kTileW) * L.n_cta * 2u);
   if (stages < kMinStagedStages) stages = fit(0u);
   p.stages = stages;
@@ -828,7 +966,7 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3((unsigned)kThreads);
+    cfg.blockDim = dim3((unsigned)(p.wstream ? kThreadsWS : kThreads));
     cfg.dynamicSmemBytes = p.smem_bytes;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -847,15 +985,21 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     using T = decltype(tag);
     constexpr bool R = decltype(ring)::value, LA = decltype(lst)::value;
     if constexpr (!R && !LA) {
-      if (p.cmajor) return go(tapconv_kernel<T, false, false, 64, true>);  // (tapconv_plan: n_cta == 64)
+      if (p.cmajor) return go(tapconv_kernel<T, false, false, 64, true, false>);  // (tapconv_plan: n_cta == 64)
+      if (p.wstream) {  // the wide ResConvs: n_cta = 96 (c = 96, 192) or 128 (c = 128)
+        if (L.n_cta == 96) return go(tapconv_kernel<T, false, false, 96, false, true>);
+        if (L.n_cta == 128) return go(tapconv_kernel<T, false, false, 128, false, true>);
+        set_error("tapconv: streamed weights are instantiated for n_cta = 96 and 128 only");
+        return cudaErrorInvalidConfiguration;
+      }
     }
     switch (L.n_cta) {  // tapconv_plan admits multiples of 16 up to 96
-      case 16: return go(tapconv_kernel<T, R, LA, 16, false>);
-      case 32: return go(tapconv_kernel<T, R, LA, 32, false>);
-      case 48: return go(tapconv_kernel<T, R, LA, 48, false>);
-      case 64: return go(tapconv_kernel<T, R, LA, 64, false>);
-      case 80: return go(tapconv_kernel<T, R, LA, 80, false>);
-      default: return go(tapconv_kernel<T, R, LA, 96, false>);
+      case 16: return go(tapconv_kernel<T, R, LA, 16, false, false>);
+      case 32: return go(tapconv_kernel<T, R, LA, 32, false, false>);
+      case 48: return go(tapconv_kernel<T, R, LA, 48, false, false>);
+      case 64: return go(tapconv_kernel<T, R, LA, 64, false, false>);
+      case 80: return go(tapconv_kernel<T, R, LA, 80, false, false>);
+      default: return go(tapconv_kernel<T, R, LA, 96, false, false>);
     }
   };
   auto pick = [&](auto tag) -> cudaError_t {

@@ -67,6 +67,9 @@ struct alignas(64) TapConvParams {
   int nruns, run_len;    // MMA issue: nruns runs of run_len consecutive K=16 steps (mma[r] = first step of run r)
   int ring;              // 1: the window streams through a ring of single k-block slots (see tapconv.cu)
   int cmajor;            // 1: channel-major MMAs, the 64 output channels on the wgmma M and the tile's 128 cells on N
+  int wstream;           // 1: the weights stream through w_slots slots of four K=16 steps (see tapconv.cu)
+  int w_slots, w_groups; //    slots in shared memory / slots per tile (ceil(K16 / 4))
+  uint32_t w_slot_bytes; //    n_cta rows of 128 B
   int tiles_x, tiles_y, ntiles;
   int ctas_per_split;
   uint32_t b_hi;                  // high word of the weight (B) descriptors
@@ -89,6 +92,7 @@ struct TapConvLayer {
   int halo_y0 = 0, halo_x0 = 0, halo_h = 0, halo_w = 0;
   int epi_mode = 0, out_s2d = 0;
   int ring = 0;           // taps are listed k-block-major (kb, tap) with nk16 = 4; needs cin % 64 == 0
+  int wstream = 0;        // streamed weights, whole window per tile (ResConv, n_cta 96 / 128; see tapconv.cu)
   TapEntry taps[kMaxTaps];
   void* w = nullptr;      // device
   float* shift = nullptr; // device

@@ -158,11 +158,11 @@ class Rife46Engine:
         return out
 
     def layer_plan(self, block, layer):
-        st, nc, ns, sm, mc, cm = C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int64(), C.c_int()
+        st, nc, ns, sm, mc, cm, ws = C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int64(), C.c_int(), C.c_int()
         check(self._L.vfi_rife46_layer_plan(self._ctx, block, layer, C.byref(st), C.byref(nc), C.byref(ns),
-                                            C.byref(sm), C.byref(mc), C.byref(cm)))
+                                            C.byref(sm), C.byref(mc), C.byref(cm), C.byref(ws)))
         return dict(stages=st.value, n_cta=nc.value, nsplit=ns.value, smem_bytes=sm.value, macs_per_cell=mc.value,
-                    cmajor=bool(cm.value))
+                    cmajor=bool(cm.value), wstream=bool(ws.value))
 
     def debug_state(self, batch):
         """(flow [B,Hp,Wp,4], mask [B,Hp,Wp]) of the last internal pass as torch CUDA tensors."""

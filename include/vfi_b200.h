@@ -217,9 +217,10 @@ int vfi_rife46_debug_layer(vfi_ctx* ctx, int block, int layer, const void* in, v
  * pass into caller-provided DEVICE buffers (either may be NULL to only query Hp/Wp); synchronises. */
 int vfi_rife46_debug_state(vfi_ctx* ctx, float* flow4_out, float* mask_out, int batch, int* Hp, int* Wp);
 /* Static plan of a layer for (block, layer): shared-memory stages, CTA output channels, splits, smem bytes, MACs per
- * grid cell, and cmajor = 1 when the layer runs channel-major (output channels on the MMA's M, 128 cells on N). */
+ * grid cell, cmajor = 1 when the layer runs channel-major (output channels on the MMA's M, 128 cells on N) and
+ * wstream = 1 when its weights stream through shared memory instead of staying resident (any pointer may be NULL). */
 int vfi_rife46_layer_plan(vfi_ctx* ctx, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
-                          int64_t* macs_per_cell, int* cmajor);
+                          int64_t* macs_per_cell, int* cmajor, int* wstream);
 int vfi_sync(vfi_ctx* ctx);
 
 /* Measurement hook (bench.py's roofline lines): while enabled, every internal pass of the RIFE forward schedule records
