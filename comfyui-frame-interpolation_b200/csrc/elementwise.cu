@@ -1,11 +1,13 @@
 // Full-resolution, HBM-bound kernels of the RIFE-4.6 path (fp32 flow / mask / image arithmetic):
 //   prep_frames : clamp(0,1) + zero-pad to x64 + RGB->float4           rife_arch.py:476-485
-//   front       : [warp(img0), warp(img1), t, mask, flow] -> bilinear 1/s -> 16-channel block input, written
-//                 directly in the space-to-depth form the stride-2 conv0.0 reads
+//   front       : [warp(img0), warp(img1), (features), t, mask, flow] -> bilinear 1/s or k-times up -> block input
+//                 of the arch's Layout, written directly in the space-to-depth form the stride-2 conv0.0 reads
 //                                                                       rife_arch.py:31-70, :238-249, :589-596
 //   (flow)      : flow = sum_j up_sj(T_j)*s_j is evaluated on the fly from the blocks' low-res outputs   rife_arch.py:263-266, :694-696
 //   final       : warp both frames with the final flow, sigmoid blend, crop, clamp    rife_arch.py:703-704, :713-717, :732
 //   warp        : stand-alone backward bilinear warp (border, align_corners=True), NHWC fp32, any C
+#include <type_traits>
+
 #include "ptx.cuh"
 #include "vfi_internal.h"
 
@@ -197,77 +199,24 @@ __device__ __forceinline__ void flow_at(const FlowLevels& L, int b, int Hp, int 
   }
 }
 
-// one thread = one cell of the 1/s grid; channels: w0.rgb, w1.rgb, t, mask, flow/s (4) [, 4 zero pad].
-// Thread order (b, row pair, x, row parity) so that 4 consecutive lanes fill one 128-byte space-to-depth cell.
-template <typename T, int NLEV, int S>
-__global__ void front_kernel(const uint2* __restrict__ imgs, const FlowLevels lev, const BatchTasks tasks, int Hp,
-                             int Wp, int s_rt, T* __restrict__ x_s2d) {
-  const int s = S ? S : s_rt;
-  const int Hs = Hp / s, Ws = Wp / s;
-  const size_t plane = (size_t)Hp * Wp;
-  const float inv_s = 1.f / (float)s;
-  // grid = (x cells / 64, row pairs, images): no 64-bit integer division of a flat index per thread
-  {
-    const int par = (int)(threadIdx.x & 1);
-    const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-    if (xl >= Ws) return;
-    const int yl = (int)blockIdx.y * 2 + par;
-    const int b = (int)blockIdx.z;
-    const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-    const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-    const float t = tasks.t[b];
-    // bilinear 1/s, align_corners=False: the two source taps per axis are s*i + s/2 - 1 and s*i + s/2, weight 1/2
-    const int ntap = (s == 1) ? 1 : 2;
-    const int by = (s == 1) ? yl : s * yl + s / 2 - 1;
-    const int bx = (s == 1) ? xl : s * xl + s / 2 - 1;
-    float ch[12];
-    float rowacc[2][12];
+// Space-to-depth store of a block input: cell (yl, xl) of the [Hs][Ws] grid -> [b, yl/2, xl/2, ((yl&1)*2 + (xl&1))*SUB + c]
+// as SUB/8 uint4, the channels past C zero.  The front kernels order their threads (b, row pair, x, row parity), so 4
+// consecutive lanes fill one 4*SUB-channel cell.
+template <typename T, int C, int SUB>
+__device__ __forceinline__ void store_s2d(T* __restrict__ x_s2d, int b, int Hs, int Ws, int yl, int xl,
+                                          const float (&ch)[C]) {
+  static_assert(C % 2 == 0 && C <= SUB && SUB % 8 == 0, "whole channel pairs inside the sub-cell");
+  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
+  uint4* dst = reinterpret_cast<uint4*>(x_s2d + cell * (4 * SUB) + ((yl & 1) * 2 + (xl & 1)) * SUB);
 #pragma unroll
-    for (int ty = 0; ty < 2; ++ty) {
-      float colv[2][12];
+  for (int q = 0; q < SUB / 8; ++q) {
+    uint32_t w[4];
 #pragma unroll
-      for (int tx = 0; tx < 2; ++tx) {
-        if (ty < ntap && tx < ntap) {
-          const int Y = by + ty, X = bx + tx;
-          float* v = colv[tx];
-          if (NLEV == 0) {
-            const float4 a = unpack_h4(__ldg(img0 + (size_t)Y * Wp + X));
-            const float4 c = unpack_h4(__ldg(img1 + (size_t)Y * Wp + X));
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
-            v[6] = t; v[7] = 0.f; v[8] = 0.f; v[9] = 0.f; v[10] = 0.f; v[11] = 0.f;
-          } else {
-            float4 f;
-            float m;
-            flow_at<(NLEV > 0 ? NLEV : 1)>(lev, b, Hp, Wp, Y, X, f, m);
-            const float4 a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-            const float4 c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
-            v[6] = t; v[7] = m; v[8] = f.x; v[9] = f.y; v[10] = f.z; v[11] = f.w;
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) rowacc[ty][i] = (ntap == 1) ? colv[0][i] : (colv[0][i] + colv[1][i]);
+    for (int j = 0; j < 4; ++j) {
+      const int c = 8 * q + 2 * j;
+      w[j] = c < C ? Pack2<T>::pack(ch[c], ch[c + 1]) : 0u;
     }
-#pragma unroll
-    for (int i = 0; i < 12; ++i) ch[i] = (ntap == 1) ? rowacc[0][i] : 0.25f * (rowacc[0][i] + rowacc[1][i]);
-#pragma unroll
-    for (int i = 8; i < 12; ++i) ch[i] *= inv_s;  // flow is also divided by the scale (rife_arch.py:242-248)
-
-    // space-to-depth store: cell (yl, xl) -> [b, yl/2, xl/2, ((yl&1)*2 + (xl&1))*16 + c]
-    const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-    T* dst = x_s2d + cell * 64 + ((yl & 1) * 2 + (xl & 1)) * 16;
-    uint4 lo, hi;
-    lo.x = Pack2<T>::pack(ch[0], ch[1]);
-    lo.y = Pack2<T>::pack(ch[2], ch[3]);
-    lo.z = Pack2<T>::pack(ch[4], ch[5]);
-    lo.w = Pack2<T>::pack(ch[6], ch[7]);
-    hi.x = Pack2<T>::pack(ch[8], ch[9]);
-    hi.y = Pack2<T>::pack(ch[10], ch[11]);
-    hi.z = 0u;
-    hi.w = 0u;
-    reinterpret_cast<uint4*>(dst)[0] = lo;
-    reinterpret_cast<uint4*>(dst)[1] = hi;
+    dst[q] = make_uint4(w[0], w[1], w[2], w[3]);
   }
 }
 
@@ -390,19 +339,7 @@ __global__ void front2_kernel(const uint2* __restrict__ imgs, const FlowLevels l
         lev.out_m[pid] = m[q];
       }
     }
-    const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-    T* dst = x_s2d + cell * 64 + ((yl & 1) * 2 + (xl & 1)) * 16;
-    uint4 lo, hi;
-    lo.x = Pack2<T>::pack(ch[0], ch[1]);
-    lo.y = Pack2<T>::pack(ch[2], ch[3]);
-    lo.z = Pack2<T>::pack(ch[4], ch[5]);
-    lo.w = Pack2<T>::pack(ch[6], ch[7]);
-    hi.x = Pack2<T>::pack(ch[8], ch[9]);
-    hi.y = Pack2<T>::pack(ch[10], ch[11]);
-    hi.z = 0u;
-    hi.w = 0u;
-    reinterpret_cast<uint4*>(dst)[0] = lo;
-    reinterpret_cast<uint4*>(dst)[1] = hi;
+    store_s2d<T, 12, 16>(x_s2d, b, Hs, Ws, yl, xl, ch);
   }
 }
 
@@ -494,86 +431,6 @@ __global__ void encode_deconv_kernel(const float* __restrict__ e16, const float*
   }
 }
 
-// arch 4.7 block input: [w0.rgb, w1.rgb, warp(f0) (4), warp(f1) (4), t, mask, flow/s (4)] = 20 of 32 channels
-// (block 0: [img0, img1, f0, f1, t] = 15), space-to-depth cell = 4 x 32 channels
-template <typename T, int NLEV>
-__global__ void front47_kernel(const uint2* __restrict__ imgs, const uint2* __restrict__ feats,
-                               const FlowLevels lev, const BatchTasks tasks, int Hp, int Wp, int s,
-                               T* __restrict__ x_s2d) {
-  const int Hs = Hp / s, Ws = Wp / s;
-  const size_t plane = (size_t)Hp * Wp;
-  const float inv_s = 1.f / (float)s;
-  {
-    const int par = (int)(threadIdx.x & 1);
-    const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-    if (xl >= Ws) return;
-    const int yl = (int)blockIdx.y * 2 + par;
-    const int b = (int)blockIdx.z;
-    const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;  // half4 planes: the block input is 16-bit anyway
-    const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-    const uint2* ft0 = feats + (size_t)tasks.f0[b] * plane;
-    const uint2* ft1 = feats + (size_t)tasks.f1[b] * plane;
-    const float t = tasks.t[b];
-    const int ntap = (s == 1) ? 1 : 2;
-    const int by = (s == 1) ? yl : s * yl + s / 2 - 1;
-    const int bx = (s == 1) ? xl : s * xl + s / 2 - 1;
-    float ch[20];
-#pragma unroll
-    for (int i = 0; i < 20; ++i) ch[i] = 0.f;
-    float rowacc[2][20];
-#pragma unroll
-    for (int ty = 0; ty < 2; ++ty) {
-      float colv[2][20];
-#pragma unroll
-      for (int tx = 0; tx < 2; ++tx) {
-        if (ty < ntap && tx < ntap) {
-          const int Y = by + ty, X = bx + tx;
-          float* v = colv[tx];
-          float4 a, c, fa, fc;
-          if (NLEV == 0) {
-            a = unpack_h4(__ldg(img0 + (size_t)Y * Wp + X));
-            c = unpack_h4(__ldg(img1 + (size_t)Y * Wp + X));
-            fa = unpack_h4(__ldg(ft0 + (size_t)Y * Wp + X));
-            fc = unpack_h4(__ldg(ft1 + (size_t)Y * Wp + X));
-            v[14] = t; v[15] = 0.f; v[16] = 0.f; v[17] = 0.f; v[18] = 0.f; v[19] = 0.f;
-          } else {
-            float4 f;
-            float m;
-            flow_at<(NLEV > 0 ? NLEV : 1)>(lev, b, Hp, Wp, Y, X, f, m);
-            a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-            c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-            fa = sample_border4(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-            fc = sample_border4(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-            v[14] = t; v[15] = m; v[16] = f.x; v[17] = f.y; v[18] = f.z; v[19] = f.w;
-          }
-          v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
-          v[6] = fa.x; v[7] = fa.y; v[8] = fa.z; v[9] = fa.w; v[10] = fc.x; v[11] = fc.y; v[12] = fc.z; v[13] = fc.w;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 20; ++i) rowacc[ty][i] = (ntap == 1) ? colv[0][i] : (colv[0][i] + colv[1][i]);
-    }
-#pragma unroll
-    for (int i = 0; i < 20; ++i) ch[i] = (ntap == 1) ? rowacc[0][i] : 0.25f * (rowacc[0][i] + rowacc[1][i]);
-#pragma unroll
-    for (int i = 16; i < 20; ++i) ch[i] *= inv_s;
-    const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-    T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-    uint4 q0, q1, q2;
-    q0.x = Pack2<T>::pack(ch[0], ch[1]);   q0.y = Pack2<T>::pack(ch[2], ch[3]);
-    q0.z = Pack2<T>::pack(ch[4], ch[5]);   q0.w = Pack2<T>::pack(ch[6], ch[7]);
-    q1.x = Pack2<T>::pack(ch[8], ch[9]);   q1.y = Pack2<T>::pack(ch[10], ch[11]);
-    q1.z = Pack2<T>::pack(ch[12], ch[13]); q1.w = Pack2<T>::pack(ch[14], ch[15]);
-    q2.x = Pack2<T>::pack(ch[16], ch[17]); q2.y = Pack2<T>::pack(ch[18], ch[19]);
-    q2.z = 0u; q2.w = 0u;
-    reinterpret_cast<uint4*>(dst)[0] = q0;
-    reinterpret_cast<uint4*>(dst)[1] = q1;
-    reinterpret_cast<uint4*>(dst)[2] = q2;
-    reinterpret_cast<uint4*>(dst)[3] = make_uint4(0u, 0u, 0u, 0u);
-  }
-}
-
-
 // ---------------------------------------------------------------------------------------------
 // arch 4.17 (rife417.pth): encode = Head_417 (rife_arch.py:356-375).  cnn0 (Conv2d 3->32, stride 2) + LeakyReLU runs
 // here on the CUDA cores (0.45 GMAC per 1080p frame) and leaves a 16-bit NHWC [Hh][Wh][32] tensor for the tensor-core
@@ -652,100 +509,11 @@ __device__ __forceinline__ void sample_border8(const uint4* __restrict__ ft, int
   for (int i = 0; i < 8; ++i) o[i] = a[i] * w00 + b[i] * w01 + c[i] * w10 + d[i] * w11;
 }
 
-// arch 4.17 block input: [w0.rgb, w1.rgb, warp(f0) (8), warp(f1) (8), t, mask, flow/s (4)] = 28 of 32 channels
-// (block 0: [img0, img1, f0, f1, t] = 23), space-to-depth cell = 4 x 32 channels.  Same structure as front47_kernel;
-// the 2x2 centre taps are summed row by row in the reference's order ((a + b) + (c + d)) * 0.25.
-template <typename T, int NLEV>
-__global__ void front417_kernel(const uint2* __restrict__ imgs, const uint4* __restrict__ feats,
-                                const FlowLevels lev, const BatchTasks tasks, int Hp, int Wp, int s,
-                                T* __restrict__ x_s2d) {
-  const int Hs = Hp / s, Ws = Wp / s;
-  const size_t plane = (size_t)Hp * Wp;
-  const size_t fplane = plane / 4 * 4;  // uint4 per pixel: (Hp/2)*(Wp/2) cells x 4
-  const float inv_s = 1.f / (float)s;
-  const int par = (int)(threadIdx.x & 1);
-  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-  if (xl >= Ws) return;
-  const int yl = (int)blockIdx.y * 2 + par;
-  const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;  // half4 planes: the block input is 16-bit anyway
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const uint4* ft0 = feats + (size_t)tasks.f0[b] * fplane;
-  const uint4* ft1 = feats + (size_t)tasks.f1[b] * fplane;
-  const float t = tasks.t[b];
-  const int ntap = (s == 1) ? 1 : 2;
-  const int by = (s == 1) ? yl : s * yl + s / 2 - 1;
-  const int bx = (s == 1) ? xl : s * xl + s / 2 - 1;
-  float ch[28];
-#pragma unroll
-  for (int ty = 0; ty < 2; ++ty) {
-    float row[28];
-#pragma unroll
-    for (int tx = 0; tx < 2; ++tx) {
-      if (ty < ntap && tx < ntap) {
-        const int Y = by + ty, X = bx + tx;
-        float v[28];
-        float4 a, c;
-        float fa[8], fc[8];
-        if (NLEV == 0) {
-          a = unpack_h4(__ldg(img0 + (size_t)Y * Wp + X));
-          c = unpack_h4(__ldg(img1 + (size_t)Y * Wp + X));
-          load_feat8<T>(ft0, Wp >> 1, Y, X, fa);
-          load_feat8<T>(ft1, Wp >> 1, Y, X, fc);
-          v[22] = t; v[23] = 0.f; v[24] = 0.f; v[25] = 0.f; v[26] = 0.f; v[27] = 0.f;
-        } else {
-          float4 f;
-          float m;
-          flow_at<(NLEV > 0 ? NLEV : 1)>(lev, b, Hp, Wp, Y, X, f, m);
-          a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-          c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-          sample_border8<T>(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y, fa);
-          sample_border8<T>(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w, fc);
-          v[22] = t; v[23] = m; v[24] = f.x; v[25] = f.y; v[26] = f.z; v[27] = f.w;
-        }
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          v[6 + i] = fa[i];
-          v[14 + i] = fc[i];
-        }
-#pragma unroll
-        for (int i = 0; i < 28; ++i) row[i] = (tx == 0) ? v[i] : row[i] + v[i];
-      }
-    }
-    if (ty < ntap) {
-#pragma unroll
-      for (int i = 0; i < 28; ++i) ch[i] = (ty == 0) ? row[i] : ch[i] + row[i];
-    }
-  }
-  if (ntap == 2) {
-#pragma unroll
-    for (int i = 0; i < 28; ++i) ch[i] *= 0.25f;
-  }
-#pragma unroll
-  for (int i = 24; i < 28; ++i) ch[i] *= inv_s;  // flow is also divided by the scale (rife_arch.py:242-248)
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-  uint4 q[4];
-  q[0] = make_uint4(Pack2<T>::pack(ch[0], ch[1]), Pack2<T>::pack(ch[2], ch[3]), Pack2<T>::pack(ch[4], ch[5]),
-                    Pack2<T>::pack(ch[6], ch[7]));
-  q[1] = make_uint4(Pack2<T>::pack(ch[8], ch[9]), Pack2<T>::pack(ch[10], ch[11]), Pack2<T>::pack(ch[12], ch[13]),
-                    Pack2<T>::pack(ch[14], ch[15]));
-  q[2] = make_uint4(Pack2<T>::pack(ch[16], ch[17]), Pack2<T>::pack(ch[18], ch[19]), Pack2<T>::pack(ch[20], ch[21]),
-                    Pack2<T>::pack(ch[22], ch[23]));
-  q[3] = make_uint4(Pack2<T>::pack(ch[24], ch[25]), Pack2<T>::pack(ch[26], ch[27]), 0u, 0u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) reinterpret_cast<uint4*>(dst)[i] = q[i];
-}
-
 // ---------------------------------------------------------------------------------------------
 // arch 4.26 (rife426.pth): encode = Head (rife_arch.py:378-395; cnn0 on the CUDA cores via head0_kernel with the 16
 // output channels zero-padded to 32, cnn1..cnn3 as tapconv layers) -> 4-channel 16-bit features stored space-to-depth
-// ([Hh][Wh][4 x 4]: one uint2 per pixel).  Block input (rife_arch.py:521-526, :563-587):
-//   block 0 : [img0, img1, f0 (4), f1 (4), t]                                                        = 15 of 32 channels
-//   block i : [w0.rgb, w1.rgb, warp(f0), warp(f1), t, mask, feat (8), flow/s (4)]                     = 28 of 32 channels
-// where `feat` = the previous block's 8 extra lastconv channels, bilinearly up-scaled to full resolution by its scale
-// (rife_arch.py:267-274) and, like every other channel, down-scaled by 1/s here (2x2 centre taps).
+// ([Hh][Wh][4 x 4]: one uint2 per pixel).  Its block input also carries the previous block's 8 extra lastconv channels,
+// brought to full resolution by up_feat8 / down_feat8 (rife_arch.py:267-274).
 // ---------------------------------------------------------------------------------------------
 template <typename T>
 __device__ __forceinline__ void load_feat4(const uint2* __restrict__ ft, int Wh, int Y, int X, float (&v)[4]) {
@@ -803,282 +571,6 @@ __device__ __forceinline__ void up_feat8(const uint4* __restrict__ pf, int Hs, i
   for (int i = 0; i < 8; ++i) o[i] = hy * (hx * a[i] + lx * b[i]) + ly * (hx * c[i] + lx * d[i]);
 }
 
-template <typename T, int NLEV>
-__global__ void front426_kernel(const uint2* __restrict__ imgs, const uint2* __restrict__ feats,
-                                const uint4* __restrict__ prev_feat, int prev_s, const FlowLevels lev,
-                                const BatchTasks tasks, int Hp, int Wp, int s, T* __restrict__ x_s2d) {
-  const int Hs = Hp / s, Ws = Wp / s;
-  const size_t plane = (size_t)Hp * Wp;
-  const float inv_s = 1.f / (float)s;
-  const int par = (int)(threadIdx.x & 1);
-  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-  if (xl >= Ws) return;
-  const int yl = (int)blockIdx.y * 2 + par;
-  const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const uint2* ft0 = feats + (size_t)tasks.f0[b] * plane;  // one uint2 per pixel
-  const uint2* ft1 = feats + (size_t)tasks.f1[b] * plane;
-  const int pHs = NLEV ? Hp / prev_s : 1, pWs = NLEV ? Wp / prev_s : 1;
-  const uint4* pf = NLEV ? prev_feat + (size_t)b * pHs * pWs : nullptr;
-  const float pinv = NLEV ? 1.f / (float)prev_s : 1.f;
-  const float t = tasks.t[b];
-  const int ntap = (s == 1) ? 1 : 2;
-  const int by = (s == 1) ? yl : s * yl + s / 2 - 1;
-  const int bx = (s == 1) ? xl : s * xl + s / 2 - 1;
-  float ch[28];
-#pragma unroll
-  for (int ty = 0; ty < 2; ++ty) {
-    float row[28];
-#pragma unroll
-    for (int tx = 0; tx < 2; ++tx) {
-      if (ty < ntap && tx < ntap) {
-        const int Y = by + ty, X = bx + tx;
-        float v[28];
-        float4 a, c;
-        float fa[4], fc[4];
-        if (NLEV == 0) {
-          a = unpack_h4(__ldg(img0 + (size_t)Y * Wp + X));
-          c = unpack_h4(__ldg(img1 + (size_t)Y * Wp + X));
-          load_feat4<T>(ft0, Wp >> 1, Y, X, fa);
-          load_feat4<T>(ft1, Wp >> 1, Y, X, fc);
-          v[14] = t;
-#pragma unroll
-          for (int i = 15; i < 28; ++i) v[i] = 0.f;
-        } else {
-          float4 f;
-          float m;
-          flow_at<(NLEV > 0 ? NLEV : 1)>(lev, b, Hp, Wp, Y, X, f, m);
-          a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-          c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-          sample_border4h<T>(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y, fa);
-          sample_border4h<T>(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w, fc);
-          float pe[8];
-          up_feat8<T>(pf, pHs, pWs, prev_s, pinv, Y, X, pe);
-          v[14] = t; v[15] = m;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[16 + i] = pe[i];
-          v[24] = f.x; v[25] = f.y; v[26] = f.z; v[27] = f.w;
-        }
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          v[6 + i] = fa[i];
-          v[10 + i] = fc[i];
-        }
-#pragma unroll
-        for (int i = 0; i < 28; ++i) row[i] = (tx == 0) ? v[i] : row[i] + v[i];
-      }
-    }
-    if (ty < ntap) {
-#pragma unroll
-      for (int i = 0; i < 28; ++i) ch[i] = (ty == 0) ? row[i] : ch[i] + row[i];
-    }
-  }
-  if (ntap == 2) {
-#pragma unroll
-    for (int i = 0; i < 28; ++i) ch[i] *= 0.25f;
-  }
-#pragma unroll
-  for (int i = 24; i < 28; ++i) ch[i] *= inv_s;  // flow is also divided by the scale (rife_arch.py:242-248)
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-  uint4 q[4];
-  q[0] = make_uint4(Pack2<T>::pack(ch[0], ch[1]), Pack2<T>::pack(ch[2], ch[3]), Pack2<T>::pack(ch[4], ch[5]),
-                    Pack2<T>::pack(ch[6], ch[7]));
-  q[1] = make_uint4(Pack2<T>::pack(ch[8], ch[9]), Pack2<T>::pack(ch[10], ch[11]), Pack2<T>::pack(ch[12], ch[13]),
-                    Pack2<T>::pack(ch[14], ch[15]));
-  q[2] = make_uint4(Pack2<T>::pack(ch[16], ch[17]), Pack2<T>::pack(ch[18], ch[19]), Pack2<T>::pack(ch[20], ch[21]),
-                    Pack2<T>::pack(ch[22], ch[23]));
-  q[3] = make_uint4(Pack2<T>::pack(ch[24], ch[25]), Pack2<T>::pack(ch[26], ch[27]), 0u, 0u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) reinterpret_cast<uint4*>(dst)[i] = q[i];
-}
-
-// debug / tests only: materialise the accumulated full-resolution flow and mask
-
-// ---- up-scaled blocks (node scale_factor 2 / 4: block scale 1/k, k = 2 or 4) - arch 4.6 ------------------------------
-// The reference interpolates the full-resolution block input UP by k before conv0 (rife_arch.py:238-249 with
-// scale < 1): x = interpolate(cat(warped img0, warped img1, t, mask), k), flow = interpolate(flow, k) * k, bilinear,
-// align_corners=False.  One thread = one cell of the k-times finer grid: source position (cell + 0.5) / k - 0.5 clamped at
-// 0, the four surrounding full-resolution pixels each evaluated like front_kernel does (dense flow / mask planes F, M -
-// every earlier level has been folded into them - and the two border-clamped warps), then mixed.  Same 16-channel
-// space-to-depth store as front_kernel.
-template <typename T>
-__global__ void front_up_kernel(const uint2* __restrict__ imgs, const float4* __restrict__ F, const float* __restrict__ M,
-                                const BatchTasks tasks, int Hp, int Wp, int k, T* __restrict__ x_s2d) {
-  const int Hs = Hp * k, Ws = Wp * k;
-  const size_t plane = (size_t)Hp * Wp;
-  const float inv_k = 1.f / (float)k;
-  const int par = (int)(threadIdx.x & 1);
-  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-  if (xl >= Ws) return;
-  const int yl = (int)blockIdx.y * 2 + par;
-  const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const float t = tasks.t[b];
-  const float sy = fmaxf(((float)yl + 0.5f) * inv_k - 0.5f, 0.f), sx = fmaxf(((float)xl + 0.5f) * inv_k - 0.5f, 0.f);
-  const int y0 = min((int)sy, Hp - 1), x0 = min((int)sx, Wp - 1);
-  const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
-  const float ly = sy - (float)y0, lx = sx - (float)x0;
-  const float wq[4] = {(1.f - ly) * (1.f - lx), (1.f - ly) * lx, ly * (1.f - lx), ly * lx};
-  const int qy[4] = {y0, y0, y1, y1}, qx[4] = {x0, x1, x0, x1};
-  float ch[12];
-#pragma unroll
-  for (int i = 0; i < 12; ++i) ch[i] = 0.f;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int Y = qy[q], X = qx[q];
-    const size_t pid = ((size_t)b * Hp + Y) * Wp + X;
-    const float4 f = F[pid];
-    const float m = M[pid];
-    const float4 a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-    const float4 c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-    const float v[12] = {a.x, a.y, a.z, c.x, c.y, c.z, t, m, f.x, f.y, f.z, f.w};
-#pragma unroll
-    for (int i = 0; i < 12; ++i) ch[i] = fmaf(v[i], wq[q], ch[i]);
-  }
-#pragma unroll
-  for (int i = 8; i < 12; ++i) ch[i] *= (float)k;  // flow * (1 / scale), rife_arch.py:245-248
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 64 + ((yl & 1) * 2 + (xl & 1)) * 16;
-  uint4 lo, hi;
-  lo.x = Pack2<T>::pack(ch[0], ch[1]);
-  lo.y = Pack2<T>::pack(ch[2], ch[3]);
-  lo.z = Pack2<T>::pack(ch[4], ch[5]);
-  lo.w = Pack2<T>::pack(ch[6], ch[7]);
-  hi.x = Pack2<T>::pack(ch[8], ch[9]);
-  hi.y = Pack2<T>::pack(ch[10], ch[11]);
-  hi.z = 0u;
-  hi.w = 0u;
-  reinterpret_cast<uint4*>(dst)[0] = lo;
-  reinterpret_cast<uint4*>(dst)[1] = hi;
-}
-
-// arch 4.7 variant: the 32-channel layout of front47_kernel ([w0.rgb, w1.rgb, warp(f0) 4, warp(f1) 4, t, mask, flow 4])
-template <typename T>
-__global__ void front_up47_kernel(const uint2* __restrict__ imgs, const uint2* __restrict__ feats, const float4* __restrict__ F,
-                                  const float* __restrict__ M, const BatchTasks tasks, int Hp, int Wp, int k,
-                                  T* __restrict__ x_s2d) {
-  const int Hs = Hp * k, Ws = Wp * k;
-  const size_t plane = (size_t)Hp * Wp;
-  const float inv_k = 1.f / (float)k;
-  const int par = (int)(threadIdx.x & 1);
-  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-  if (xl >= Ws) return;
-  const int yl = (int)blockIdx.y * 2 + par;
-  const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const uint2* ft0 = feats + (size_t)tasks.f0[b] * plane;
-  const uint2* ft1 = feats + (size_t)tasks.f1[b] * plane;
-  const float t = tasks.t[b];
-  const float sy = fmaxf(((float)yl + 0.5f) * inv_k - 0.5f, 0.f), sx = fmaxf(((float)xl + 0.5f) * inv_k - 0.5f, 0.f);
-  const int y0 = min((int)sy, Hp - 1), x0 = min((int)sx, Wp - 1);
-  const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
-  const float ly = sy - (float)y0, lx = sx - (float)x0;
-  const float wq[4] = {(1.f - ly) * (1.f - lx), (1.f - ly) * lx, ly * (1.f - lx), ly * lx};
-  const int qy[4] = {y0, y0, y1, y1}, qx[4] = {x0, x1, x0, x1};
-  float ch[20];
-#pragma unroll
-  for (int i = 0; i < 20; ++i) ch[i] = 0.f;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int Y = qy[q], X = qx[q];
-    const size_t pid = ((size_t)b * Hp + Y) * Wp + X;
-    const float4 f = F[pid];
-    const float m = M[pid];
-    const float4 a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-    const float4 c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-    const float4 fa = sample_border4(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-    const float4 fc = sample_border4(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-    const float v[20] = {a.x, a.y, a.z, c.x, c.y, c.z, fa.x, fa.y, fa.z, fa.w, fc.x, fc.y, fc.z, fc.w, t, m, f.x, f.y, f.z, f.w};
-#pragma unroll
-    for (int i = 0; i < 20; ++i) ch[i] = fmaf(v[i], wq[q], ch[i]);
-  }
-#pragma unroll
-  for (int i = 16; i < 20; ++i) ch[i] *= (float)k;
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-  uint4 q0, q1, q2;
-  q0.x = Pack2<T>::pack(ch[0], ch[1]);   q0.y = Pack2<T>::pack(ch[2], ch[3]);
-  q0.z = Pack2<T>::pack(ch[4], ch[5]);   q0.w = Pack2<T>::pack(ch[6], ch[7]);
-  q1.x = Pack2<T>::pack(ch[8], ch[9]);   q1.y = Pack2<T>::pack(ch[10], ch[11]);
-  q1.z = Pack2<T>::pack(ch[12], ch[13]); q1.w = Pack2<T>::pack(ch[14], ch[15]);
-  q2.x = Pack2<T>::pack(ch[16], ch[17]); q2.y = Pack2<T>::pack(ch[18], ch[19]);
-  q2.z = 0u; q2.w = 0u;
-  reinterpret_cast<uint4*>(dst)[0] = q0;
-  reinterpret_cast<uint4*>(dst)[1] = q1;
-  reinterpret_cast<uint4*>(dst)[2] = q2;
-  reinterpret_cast<uint4*>(dst)[3] = make_uint4(0u, 0u, 0u, 0u);
-}
-
-// arch 4.17 variant: the 32-channel layout of front417_kernel ([w0.rgb, w1.rgb, warp(f0) 8, warp(f1) 8, t, mask, flow 4])
-template <typename T>
-__global__ void front_up417_kernel(const uint2* __restrict__ imgs, const uint4* __restrict__ feats, const float4* __restrict__ F,
-                                   const float* __restrict__ M, const BatchTasks tasks, int Hp, int Wp, int k,
-                                   T* __restrict__ x_s2d) {
-  const int Hs = Hp * k, Ws = Wp * k;
-  const size_t plane = (size_t)Hp * Wp;
-  const size_t fplane = plane / 4 * 4;
-  const float inv_k = 1.f / (float)k;
-  const int par = (int)(threadIdx.x & 1);
-  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
-  if (xl >= Ws) return;
-  const int yl = (int)blockIdx.y * 2 + par;
-  const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const uint4* ft0 = feats + (size_t)tasks.f0[b] * fplane;
-  const uint4* ft1 = feats + (size_t)tasks.f1[b] * fplane;
-  const float t = tasks.t[b];
-  const float sy = fmaxf(((float)yl + 0.5f) * inv_k - 0.5f, 0.f), sx = fmaxf(((float)xl + 0.5f) * inv_k - 0.5f, 0.f);
-  const int y0 = min((int)sy, Hp - 1), x0 = min((int)sx, Wp - 1);
-  const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
-  const float ly = sy - (float)y0, lx = sx - (float)x0;
-  const float wq[4] = {(1.f - ly) * (1.f - lx), (1.f - ly) * lx, ly * (1.f - lx), ly * lx};
-  const int qy[4] = {y0, y0, y1, y1}, qx[4] = {x0, x1, x0, x1};
-  float ch[28];
-#pragma unroll
-  for (int i = 0; i < 28; ++i) ch[i] = 0.f;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int Y = qy[q], X = qx[q];
-    const size_t pid = ((size_t)b * Hp + Y) * Wp + X;
-    const float4 f = F[pid];
-    const float m = M[pid];
-    const float4 a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-    const float4 c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-    float fa[8], fc[8];
-    sample_border8<T>(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y, fa);
-    sample_border8<T>(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w, fc);
-    float v[28] = {a.x, a.y, a.z, c.x, c.y, c.z};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      v[6 + i] = fa[i];
-      v[14 + i] = fc[i];
-    }
-    v[22] = t; v[23] = m; v[24] = f.x; v[25] = f.y; v[26] = f.z; v[27] = f.w;
-#pragma unroll
-    for (int i = 0; i < 28; ++i) ch[i] = fmaf(v[i], wq[q], ch[i]);
-  }
-#pragma unroll
-  for (int i = 24; i < 28; ++i) ch[i] *= (float)k;
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-  uint4 q4[4];
-  q4[0] = make_uint4(Pack2<T>::pack(ch[0], ch[1]), Pack2<T>::pack(ch[2], ch[3]), Pack2<T>::pack(ch[4], ch[5]),
-                     Pack2<T>::pack(ch[6], ch[7]));
-  q4[1] = make_uint4(Pack2<T>::pack(ch[8], ch[9]), Pack2<T>::pack(ch[10], ch[11]), Pack2<T>::pack(ch[12], ch[13]),
-                     Pack2<T>::pack(ch[14], ch[15]));
-  q4[2] = make_uint4(Pack2<T>::pack(ch[16], ch[17]), Pack2<T>::pack(ch[18], ch[19]), Pack2<T>::pack(ch[20], ch[21]),
-                     Pack2<T>::pack(ch[22], ch[23]));
-  q4[3] = make_uint4(Pack2<T>::pack(ch[24], ch[25]), Pack2<T>::pack(ch[26], ch[27]), 0u, 0u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) reinterpret_cast<uint4*>(dst)[i] = q4[i];
-}
-
 // interpolate(scale_factor = 1 / k) of an 8-channel plane pf [k Hp][k Wp] at full-res (Y, X): the two central taps per axis
 template <typename T>
 __device__ __forceinline__ void down_feat8(const uint4* __restrict__ pf, int Ws, int k, int Y, int X, float (&o)[8]) {
@@ -1092,76 +584,206 @@ __device__ __forceinline__ void down_feat8(const uint4* __restrict__ pf, int Ws,
   for (int i = 0; i < 8; ++i) o[i] = 0.5f * (0.5f * a[i] + 0.5f * b[i]) + 0.5f * (0.5f * c[i] + 0.5f * d[i]);
 }
 
-// arch 4.26 variant: the layout of front426_kernel ([w0.rgb, w1.rgb, warp(f0) 4, warp(f1) 4, t, mask, feat 8, flow 4]); `feat`
-// = the previous block's 8 extra lastconv channels brought to full resolution (up by its scale prev_s, or - when that block
-// was itself up-scaled by prev_k - down by prev_k; rife_arch.py:267-274), then up-scaled with everything else.
-template <typename T>
-__global__ void front_up426_kernel(const uint2* __restrict__ imgs, const uint2* __restrict__ feats,
-                                   const uint4* __restrict__ prev_feat, int prev_s, int prev_k, const float4* __restrict__ F,
-                                   const float* __restrict__ M, const BatchTasks tasks, int Hp, int Wp, int k,
-                                   T* __restrict__ x_s2d) {
+// ---------------------------------------------------------------------------------------------
+// Block input of every arch (rife_arch.py:238-249, :501-526, :563-587).  Each full-resolution pixel gives the channels
+//     [w0.rgb, w1.rgb, feat0 (F), feat1 (F), t, mask, prev_feat (P), flow (4)]
+// warped at the accumulated flow; block 0 takes the raw frames and features, with mask, prev_feat and flow zero.  The block
+// input is stored space-to-depth in sub-cells of SUB channels, the unused ones zero:
+//     arch  F  P  channels  SUB  features of one frame
+//     4.6   0  0     12      16
+//     4.7   4  0     20      32  half4 plane [Hp][Wp] (encode_deconv_kernel)
+//     4.17  8  0     28      32  16-bit space-to-depth [Hh][Wh][4 x 8] (Head_417)
+//     4.26  4  8     28      32  16-bit space-to-depth [Hh][Wh][4 x 4] (Head); prev_feat: the previous block's 8 extra
+//                                lastconv channels [B][pHs][pWs] at its scale, or k times finer when it was up-scaled by k
+// ---------------------------------------------------------------------------------------------
+template <int ARCH>
+struct Layout {
+  static constexpr int F = ARCH == 46 ? 0 : (ARCH == 417 ? 8 : 4);
+  static constexpr int P = ARCH == 426 ? 8 : 0;
+  static constexpr int C = 12 + 2 * F + P;
+  static constexpr int SUB = C > 16 ? 32 : 16;
+  using Feat = typename std::conditional<ARCH == 417, uint4, uint2>::type;  // one per full-resolution pixel
+
+  // where image b's block input is gathered from
+  struct Src {
+    const uint2* img0;  // half4 planes: the block input is 16-bit anyway
+    const uint2* img1;
+    const Feat* ft0;
+    const Feat* ft1;
+    const uint4* pf;
+    int pHs, pWs, prev_s, prev_k;
+    float pinv;
+    float t;
+  };
+
+  static __device__ __forceinline__ Src src(const uint2* imgs, const void* feats, const uint4* prev_feat, int prev_s,
+                                            int prev_k, const BatchTasks& tasks, int b, int Hp, int Wp) {
+    const size_t plane = (size_t)Hp * Wp;
+    Src r{};
+    r.img0 = imgs + (size_t)tasks.f0[b] * plane;
+    r.img1 = imgs + (size_t)tasks.f1[b] * plane;
+    if (F > 0) {
+      r.ft0 = static_cast<const Feat*>(feats) + (size_t)tasks.f0[b] * plane;
+      r.ft1 = static_cast<const Feat*>(feats) + (size_t)tasks.f1[b] * plane;
+    }
+    if (P > 0 && prev_feat != nullptr) {
+      r.prev_s = prev_s;
+      r.prev_k = prev_k;
+      r.pHs = prev_k > 1 ? Hp * prev_k : Hp / prev_s;
+      r.pWs = prev_k > 1 ? Wp * prev_k : Wp / prev_s;
+      r.pinv = 1.f / (float)prev_s;
+      r.pf = prev_feat + (size_t)b * r.pHs * r.pWs;
+    }
+    r.t = tasks.t[b];
+    return r;
+  }
+
+  // the channels of full-resolution pixel (Y, X): raw (WARP false, block 0) or warped by flow f, with mask m
+  template <typename T, bool WARP>
+  static __device__ __forceinline__ void pixel(const Src& s, int Hp, int Wp, int Y, int X, float4 f, float m,
+                                               float (&v)[C]) {
+    const float x0 = (float)X + f.x, y0 = (float)Y + f.y, x1 = (float)X + f.z, y1 = (float)Y + f.w;
+    const float4 a = WARP ? sample_border(s.img0, Hp, Wp, x0, y0) : unpack_h4(__ldg(s.img0 + (size_t)Y * Wp + X));
+    const float4 c = WARP ? sample_border(s.img1, Hp, Wp, x1, y1) : unpack_h4(__ldg(s.img1 + (size_t)Y * Wp + X));
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = c.x; v[4] = c.y; v[5] = c.z;
+    if constexpr (F > 0) {
+      float fa[F], fc[F];
+      if constexpr (ARCH == 47) {
+        const float4 qa = WARP ? sample_border4(s.ft0, Hp, Wp, x0, y0) : unpack_h4(__ldg(s.ft0 + (size_t)Y * Wp + X));
+        const float4 qc = WARP ? sample_border4(s.ft1, Hp, Wp, x1, y1) : unpack_h4(__ldg(s.ft1 + (size_t)Y * Wp + X));
+        fa[0] = qa.x; fa[1] = qa.y; fa[2] = qa.z; fa[3] = qa.w;
+        fc[0] = qc.x; fc[1] = qc.y; fc[2] = qc.z; fc[3] = qc.w;
+      } else if constexpr (ARCH == 417) {
+        if (WARP) {
+          sample_border8<T>(s.ft0, Hp, Wp, x0, y0, fa);
+          sample_border8<T>(s.ft1, Hp, Wp, x1, y1, fc);
+        } else {
+          load_feat8<T>(s.ft0, Wp >> 1, Y, X, fa);
+          load_feat8<T>(s.ft1, Wp >> 1, Y, X, fc);
+        }
+      } else {
+        if (WARP) {
+          sample_border4h<T>(s.ft0, Hp, Wp, x0, y0, fa);
+          sample_border4h<T>(s.ft1, Hp, Wp, x1, y1, fc);
+        } else {
+          load_feat4<T>(s.ft0, Wp >> 1, Y, X, fa);
+          load_feat4<T>(s.ft1, Wp >> 1, Y, X, fc);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < F; ++i) {
+        v[6 + i] = fa[i];
+        v[6 + F + i] = fc[i];
+      }
+    }
+    v[6 + 2 * F] = s.t;
+    v[7 + 2 * F] = WARP ? m : 0.f;
+    if constexpr (P > 0) {
+      float pe[P] = {};
+      if (WARP) {
+        if (s.prev_k > 1)
+          down_feat8<T>(s.pf, s.pWs, s.prev_k, Y, X, pe);
+        else
+          up_feat8<T>(s.pf, s.pHs, s.pWs, s.prev_s, s.pinv, Y, X, pe);
+      }
+#pragma unroll
+      for (int i = 0; i < P; ++i) v[8 + 2 * F + i] = pe[i];
+    }
+    v[C - 4] = WARP ? f.x : 0.f;
+    v[C - 3] = WARP ? f.y : 0.f;
+    v[C - 2] = WARP ? f.z : 0.f;
+    v[C - 1] = WARP ? f.w : 0.f;
+  }
+};
+
+// Block input at scale 1/s with NLEV levels of flow (0: block 0).  S = 1: s == 1, one tap (the pixel itself); S = 0: s = s_rt
+// >= 2, where bilinear 1/s, align_corners=False, reads the two source taps s*i + s/2 - 1 and s*i + s/2 per axis with
+// weight 1/2.  One thread = one cell of the 1/s grid.
+template <typename T, int ARCH, int NLEV, int S>
+__global__ void front_kernel(const uint2* __restrict__ imgs, const void* __restrict__ feats,
+                             const uint4* __restrict__ prev_feat, int prev_s, const FlowLevels lev,
+                             const BatchTasks tasks, int Hp, int Wp, int s_rt, T* __restrict__ x_s2d) {
+  using L = Layout<ARCH>;
+  const int s = S ? S : s_rt;
+  const int Hs = Hp / s, Ws = Wp / s;
+  const float inv_s = 1.f / (float)s;
+  // grid = (x cells / 64, row pairs, images): no 64-bit integer division of a flat index per thread
+  const int par = (int)(threadIdx.x & 1);
+  const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
+  if (xl >= Ws) return;
+  const int yl = (int)blockIdx.y * 2 + par;
+  const int b = (int)blockIdx.z;
+  const typename L::Src src = L::src(imgs, feats, NLEV > 0 ? prev_feat : nullptr, prev_s, 1, tasks, b, Hp, Wp);
+  // Block 0's taps are independent loads: a compile-time count issues all of them at once.  The warped fronts keep the
+  // run-time test, under which ptxas interleaves their flow-level and warp loads better (both measured at 1080p).
+  const int ntap = (S == 1 || (NLEV > 0 && s == 1)) ? 1 : 2;
+  const int by = (ntap == 1) ? yl : s * yl + s / 2 - 1;
+  const int bx = (ntap == 1) ? xl : s * xl + s / 2 - 1;
+  float rowacc[2][L::C];
+#pragma unroll
+  for (int ty = 0; ty < 2; ++ty) {
+    float colv[2][L::C];
+#pragma unroll
+    for (int tx = 0; tx < 2; ++tx) {
+      if (ty < ntap && tx < ntap) {
+        const int Y = by + ty, X = bx + tx;
+        float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+        float m = 0.f;
+        if constexpr (NLEV > 0) flow_at<NLEV>(lev, b, Hp, Wp, Y, X, f, m);
+        L::template pixel<T, (NLEV > 0)>(src, Hp, Wp, Y, X, f, m, colv[tx]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < L::C; ++i) rowacc[ty][i] = (ntap == 1) ? colv[0][i] : (colv[0][i] + colv[1][i]);
+  }
+  float ch[L::C];
+#pragma unroll
+  for (int i = 0; i < L::C; ++i) ch[i] = (ntap == 1) ? rowacc[0][i] : 0.25f * (rowacc[0][i] + rowacc[1][i]);
+#pragma unroll
+  for (int i = L::C - 4; i < L::C; ++i) ch[i] *= inv_s;  // flow is also divided by the scale (rife_arch.py:242-248)
+  store_s2d<T, L::C, L::SUB>(x_s2d, b, Hs, Ws, yl, xl, ch);
+}
+
+// ---- up-scaled blocks (node scale_factor 2 / 4: block scale 1/k, k = 2 or 4) ----------------------------------------
+// The reference interpolates the full-resolution block input UP by k before conv0 (rife_arch.py:238-249 with scale < 1):
+// x = interpolate(cat(...), k), flow = interpolate(flow, k) * k, bilinear, align_corners=False.  One thread = one cell of
+// the k-times finer grid: source position (cell + 0.5) / k - 0.5 clamped at 0, the four surrounding full-resolution pixels
+// each evaluated at the dense flow / mask planes F, M (every earlier level has been folded into them), then mixed.
+template <typename T, int ARCH>
+__global__ void front_up_kernel(const uint2* __restrict__ imgs, const void* __restrict__ feats,
+                                const uint4* __restrict__ prev_feat, int prev_s, int prev_k, const float4* __restrict__ F,
+                                const float* __restrict__ M, const BatchTasks tasks, int Hp, int Wp, int k,
+                                T* __restrict__ x_s2d) {
+  using L = Layout<ARCH>;
   const int Hs = Hp * k, Ws = Wp * k;
-  const size_t plane = (size_t)Hp * Wp;
-  const size_t fplane = plane / 4 * 4;
   const float inv_k = 1.f / (float)k;
   const int par = (int)(threadIdx.x & 1);
   const int xl = (int)(blockIdx.x * (blockDim.x >> 1) + (threadIdx.x >> 1));
   if (xl >= Ws) return;
   const int yl = (int)blockIdx.y * 2 + par;
   const int b = (int)blockIdx.z;
-  const uint2* img0 = imgs + (size_t)tasks.f0[b] * plane;
-  const uint2* img1 = imgs + (size_t)tasks.f1[b] * plane;
-  const uint2* ft0 = feats + (size_t)tasks.f0[b] * fplane;
-  const uint2* ft1 = feats + (size_t)tasks.f1[b] * fplane;
-  const int pHs = prev_k > 1 ? Hp * prev_k : Hp / prev_s, pWs = prev_k > 1 ? Wp * prev_k : Wp / prev_s;
-  const uint4* pf = prev_feat + (size_t)b * pHs * pWs;
-  const float pinv = 1.f / (float)prev_s;
-  const float t = tasks.t[b];
+  const typename L::Src src = L::src(imgs, feats, prev_feat, prev_s, prev_k, tasks, b, Hp, Wp);
   const float sy = fmaxf(((float)yl + 0.5f) * inv_k - 0.5f, 0.f), sx = fmaxf(((float)xl + 0.5f) * inv_k - 0.5f, 0.f);
   const int y0 = min((int)sy, Hp - 1), x0 = min((int)sx, Wp - 1);
   const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
   const float ly = sy - (float)y0, lx = sx - (float)x0;
   const float wq[4] = {(1.f - ly) * (1.f - lx), (1.f - ly) * lx, ly * (1.f - lx), ly * lx};
   const int qy[4] = {y0, y0, y1, y1}, qx[4] = {x0, x1, x0, x1};
-  float ch[28];
+  float ch[L::C];
 #pragma unroll
-  for (int i = 0; i < 28; ++i) ch[i] = 0.f;
+  for (int i = 0; i < L::C; ++i) ch[i] = 0.f;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const int Y = qy[q], X = qx[q];
     const size_t pid = ((size_t)b * Hp + Y) * Wp + X;
-    const float4 f = F[pid];
-    const float m = M[pid];
-    const float4 a = sample_border(img0, Hp, Wp, (float)X + f.x, (float)Y + f.y);
-    const float4 c = sample_border(img1, Hp, Wp, (float)X + f.z, (float)Y + f.w);
-    float fa[4], fc[4], pe[8];
-    sample_border4h<T>(ft0, Hp, Wp, (float)X + f.x, (float)Y + f.y, fa);
-    sample_border4h<T>(ft1, Hp, Wp, (float)X + f.z, (float)Y + f.w, fc);
-    if (prev_k > 1)
-      down_feat8<T>(pf, pWs, prev_k, Y, X, pe);
-    else
-      up_feat8<T>(pf, pHs, pWs, prev_s, pinv, Y, X, pe);
-    float v[28] = {a.x, a.y, a.z, c.x, c.y, c.z, fa[0], fa[1], fa[2], fa[3], fc[0], fc[1], fc[2], fc[3], t, m};
+    float v[L::C];
+    L::template pixel<T, true>(src, Hp, Wp, Y, X, F[pid], M[pid], v);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) v[16 + i] = pe[i];
-    v[24] = f.x; v[25] = f.y; v[26] = f.z; v[27] = f.w;
-#pragma unroll
-    for (int i = 0; i < 28; ++i) ch[i] = fmaf(v[i], wq[q], ch[i]);
+    for (int i = 0; i < L::C; ++i) ch[i] = fmaf(v[i], wq[q], ch[i]);
   }
 #pragma unroll
-  for (int i = 24; i < 28; ++i) ch[i] *= (float)k;
-  const size_t cell = ((size_t)b * (Hs >> 1) + (yl >> 1)) * (Ws >> 1) + (xl >> 1);
-  T* dst = x_s2d + cell * 128 + ((yl & 1) * 2 + (xl & 1)) * 32;
-  uint4 q4[4];
-  q4[0] = make_uint4(Pack2<T>::pack(ch[0], ch[1]), Pack2<T>::pack(ch[2], ch[3]), Pack2<T>::pack(ch[4], ch[5]),
-                     Pack2<T>::pack(ch[6], ch[7]));
-  q4[1] = make_uint4(Pack2<T>::pack(ch[8], ch[9]), Pack2<T>::pack(ch[10], ch[11]), Pack2<T>::pack(ch[12], ch[13]),
-                     Pack2<T>::pack(ch[14], ch[15]));
-  q4[2] = make_uint4(Pack2<T>::pack(ch[16], ch[17]), Pack2<T>::pack(ch[18], ch[19]), Pack2<T>::pack(ch[20], ch[21]),
-                     Pack2<T>::pack(ch[22], ch[23]));
-  q4[3] = make_uint4(Pack2<T>::pack(ch[24], ch[25]), Pack2<T>::pack(ch[26], ch[27]), 0u, 0u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) reinterpret_cast<uint4*>(dst)[i] = q4[i];
+  for (int i = L::C - 4; i < L::C; ++i) ch[i] *= (float)k;  // flow * (1 / scale), rife_arch.py:245-248
+  store_s2d<T, L::C, L::SUB>(x_s2d, b, Hs, Ws, yl, xl, ch);
 }
 
 // The block's output T (flow increments float4 + mask, k times finer than full resolution) back onto the dense planes:
@@ -1191,6 +813,7 @@ __global__ void fold_down_kernel(const float4* __restrict__ tf, const float* __r
   }
 }
 
+// the accumulated full-resolution flow and mask as dense planes: the fold before an up-scaled block, and the debug state
 template <int NLEV>
 __global__ void materialize_kernel(const FlowLevels lev, float4* __restrict__ flow, float* __restrict__ mask, int B,
                                    int Hp, int Wp) {
@@ -1308,76 +931,44 @@ static FlowLevels make_levels(const FlowState& fs, int lo, int hi, const float4*
   return L;
 }
 
-template <typename T>
-static void launch_front47_t(int nlev, dim3 g, cudaStream_t st, const uint2* imgs, const uint2* feats,
-                             const FlowLevels& L, const BatchTasks& tasks, int Hp, int Wp, int s, void* x) {
+template <typename T, int ARCH, int S>
+static void launch_front_ts(int nlev, dim3 g, cudaStream_t st, const uint2* imgs, const void* feats, const uint4* prev_feat,
+                            int prev_s, const FlowLevels& L, const BatchTasks& tasks, int Hp, int Wp, int s, void* x) {
   switch (nlev) {
-    case 0: VFI_LAUNCH((front47_kernel<T, 0>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 1: VFI_LAUNCH((front47_kernel<T, 1>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 2: VFI_LAUNCH((front47_kernel<T, 2>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    default: VFI_LAUNCH((front47_kernel<T, 3>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
+    case 0: VFI_LAUNCH((front_kernel<T, ARCH, 0, S>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
+    case 1: VFI_LAUNCH((front_kernel<T, ARCH, 1, S>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
+    case 2: VFI_LAUNCH((front_kernel<T, ARCH, 2, S>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
+    case 3: VFI_LAUNCH((front_kernel<T, ARCH, 3, S>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
+    default:  // the fifth block of arch 4.26
+      if constexpr (ARCH == 426)
+        VFI_LAUNCH((front_kernel<T, ARCH, 4, S>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x);
+      break;
   }
 }
 
-template <typename T>
-static void launch_front2_t(int nlev, int g, cudaStream_t st, const float4* imgs, const FlowLevels& L,
-                            const BatchTasks& tasks, int Hp, int Wp, void* x) {
-  switch (nlev) {
-    case 1: VFI_LAUNCH((front2_kernel<T, 1>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
-    case 2: VFI_LAUNCH((front2_kernel<T, 2>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
-    default: VFI_LAUNCH((front2_kernel<T, 3>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
-  }
-}
-
-template <typename T, int S>
-static void launch_front_ts(int nlev, dim3 g, cudaStream_t st, const uint2* imgs, const FlowLevels& L,
-                            const BatchTasks& tasks, int Hp, int Wp, int s, void* x) {
-  switch (nlev) {
-    case 0: VFI_LAUNCH((front_kernel<T, 0, S>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 1: VFI_LAUNCH((front_kernel<T, 1, S>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 2: VFI_LAUNCH((front_kernel<T, 2, S>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, s, (T*)x); break;
-    default: VFI_LAUNCH((front_kernel<T, 3, S>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, s, (T*)x); break;
-  }
-}
-
-template <typename T>
-static void launch_front_t(int nlev, bool shared_taps, dim3 g, cudaStream_t st, const uint2* imgs, const FlowLevels& L,
-                           const BatchTasks& tasks, int Hp, int Wp, int s, void* x) {
+template <typename T, int ARCH>
+static void launch_front_t(int nlev, bool shared_taps, dim3 g, cudaStream_t st, const uint2* imgs, const void* feats,
+                           const uint4* prev_feat, int prev_s, const FlowLevels& L, const BatchTasks& tasks, int Hp, int Wp,
+                           int s, void* x) {
   if (shared_taps) {
     switch (nlev) {
       case 1: VFI_LAUNCH((front2_kernel<T, 1>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
       case 2: VFI_LAUNCH((front2_kernel<T, 2>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
       default: VFI_LAUNCH((front2_kernel<T, 3>), g, 128, 0, st, imgs, L, tasks, Hp, Wp, (T*)x); break;
     }
-  } else if (s == 1) {
-    launch_front_ts<T, 1>(nlev, g, st, imgs, L, tasks, Hp, Wp, s, x);  // compile-time scale: 56 instead of 93 registers
+  } else if (s == 1) {  // compile-time scale: 56 instead of 93 registers (arch 4.6); front_kernel<S = 0> needs s >= 2
+    launch_front_ts<T, ARCH, 1>(nlev, g, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, x);
   } else {
-    launch_front_ts<T, 0>(nlev, g, st, imgs, L, tasks, Hp, Wp, s, x);
+    launch_front_ts<T, ARCH, 0>(nlev, g, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, x);
   }
 }
 
-template <typename T>
-static void launch_front417_t(int nlev, dim3 g, cudaStream_t st, const uint2* imgs, const uint4* feats,
-                              const FlowLevels& L, const BatchTasks& tasks, int Hp, int Wp, int s, void* x) {
-  switch (nlev) {
-    case 0: VFI_LAUNCH((front417_kernel<T, 0>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 1: VFI_LAUNCH((front417_kernel<T, 1>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 2: VFI_LAUNCH((front417_kernel<T, 2>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-    default: VFI_LAUNCH((front417_kernel<T, 3>), g, 128, 0, st, imgs, feats, L, tasks, Hp, Wp, s, (T*)x); break;
-  }
-}
-
-template <typename T>
-static void launch_front426_t(int nlev, dim3 g, cudaStream_t st, const uint2* imgs, const uint2* feats,
-                              const uint4* prev_feat, int prev_s, const FlowLevels& L, const BatchTasks& tasks, int Hp,
-                              int Wp, int s, void* x) {
-  switch (nlev) {
-    case 0: VFI_LAUNCH((front426_kernel<T, 0>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 1: VFI_LAUNCH((front426_kernel<T, 1>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 2: VFI_LAUNCH((front426_kernel<T, 2>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
-    case 3: VFI_LAUNCH((front426_kernel<T, 3>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
-    default: VFI_LAUNCH((front426_kernel<T, 4>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, L, tasks, Hp, Wp, s, (T*)x); break;
-  }
+template <typename T, int ARCH>
+static void launch_front_up_t(dim3 g, cudaStream_t st, const uint2* imgs, const void* feats, const uint4* prev_feat,
+                              int prev_s, int prev_k, const float4* F, const float* M, const BatchTasks& tasks, int Hp,
+                              int Wp, int k, void* x) {
+  VFI_LAUNCH((front_up_kernel<T, ARCH>), g, 128, 0, st, imgs, feats, prev_feat, prev_s, prev_k, F, M, tasks, Hp, Wp, k,
+             (T*)x);
 }
 
 cudaError_t launch_head0(int op_type, const float4* imgs, const float* w, const float* bias, void* out, int n, int Hp,
@@ -1390,7 +981,7 @@ cudaError_t launch_head0(int op_type, const float4* imgs, const float* w, const 
   return cudaGetLastError();
 }
 
-// block `blk` input: flow = base (if any) + levels [lo, blk); stores the accumulated flow when `store` planes given
+// arch 4.7 encode head of n frames: half4 feature planes
 cudaError_t launch_encode(const float4* imgs, const float* w0, const float* b0, const float* w1, const float* b1,
                           float* e16, uint2* feats, int n, int Hp, int Wp, cudaStream_t st) {
   const size_t t0 = (size_t)n * (Hp / 2) * (Wp / 2), t1 = (size_t)n * Hp * Wp;
@@ -1401,46 +992,31 @@ cudaError_t launch_encode(const float4* imgs, const float* w0, const float* b0, 
   return cudaGetLastError();
 }
 
-cudaError_t launch_front(int op_type, int arch, const float4* imgs, const uint2* imgs_h, const void* feats, int feat_ch,
-                         const void* prev_feat, int prev_s, const FlowState& fs, int blk, int lo, const float4* base_f, const float* base_m, float4* out_f, float* out_m, BatchTasks tasks,
-                         int Hp, int Wp, int s, void* x_s2d, cudaStream_t st) {
+// block `blk` input: flow = base (if any) + levels [lo, blk); stores the accumulated flow when `out` planes are given
+cudaError_t launch_front(int op_type, int arch, const float4* imgs, const uint2* imgs_h, const void* feats,
+                         const void* prev_feat, int prev_s, const FlowState& fs, int blk, int lo, const float4* base_f,
+                         const float* base_m, float4* out_f, float* out_m, BatchTasks tasks, int Hp, int Wp, int s,
+                         void* x_s2d, cudaStream_t st) {
   const dim3 g((unsigned)((Wp / s + 63) / 64), (unsigned)(Hp / s / 2), (unsigned)tasks.n);  // 64 cells x 2 rows per block
   const FlowLevels L = make_levels(fs, lo, blk, base_f, base_m, out_f, out_m, Hp, Wp);
   const int nlev = (blk == 0) ? 0 : (blk - lo);
-  if (blk > 0 && nlev == 0 && base_f == nullptr) return cudaErrorInvalidValue;
-  if (nlev > 4 || (arch != 426 && nlev > 3)) return cudaErrorInvalidValue;  // front kernels are built for <= 3 (4.26: 4) levels
-  if (arch == 426) {  // 4-channel 16-bit space-to-depth features + the previous block's 8 feature channels
-    if (feats == nullptr || (blk > 0 && prev_feat == nullptr)) return cudaErrorInvalidValue;
-    if (op_type == OP_BF16)
-      launch_front426_t<__nv_bfloat16>(blk == 0 ? 0 : (nlev == 0 ? 1 : nlev), g, st, imgs_h, (const uint2*)feats,
-                                       (const uint4*)prev_feat, prev_s, L, tasks, Hp, Wp, s, x_s2d);
-    else
-      launch_front426_t<__half>(blk == 0 ? 0 : (nlev == 0 ? 1 : nlev), g, st, imgs_h, (const uint2*)feats,
-                                (const uint4*)prev_feat, prev_s, L, tasks, Hp, Wp, s, x_s2d);
-    return cudaGetLastError();
-  }
-  if (feats != nullptr && feat_ch == 4) {  // arch 4.7
-    if (op_type == OP_BF16)
-      launch_front47_t<__nv_bfloat16>(blk == 0 ? 0 : nlev, g, st, imgs_h, (const uint2*)feats, L, tasks, Hp, Wp, s, x_s2d);
-    else
-      launch_front47_t<__half>(blk == 0 ? 0 : nlev, g, st, imgs_h, (const uint2*)feats, L, tasks, Hp, Wp, s, x_s2d);
-    return cudaGetLastError();
-  }
-  if (feats != nullptr) {  // arch 4.17: 8 feature channels, 16-bit, space-to-depth
-    if (op_type == OP_BF16)
-      launch_front417_t<__nv_bfloat16>(blk == 0 ? 0 : nlev, g, st, imgs_h, (const uint4*)feats, L, tasks, Hp, Wp, s, x_s2d);
-    else
-      launch_front417_t<__half>(blk == 0 ? 0 : nlev, g, st, imgs_h, (const uint4*)feats, L, tasks, Hp, Wp, s, x_s2d);
-    return cudaGetLastError();
-  }
-  // scale-2 front without a base plane whose levels are all at scale 4, 8, ...: the level taps are shared per cell
-  bool shared_taps = (s == 2 && blk > 0 && base_f == nullptr && nlev >= 1);
+  if (blk > 0 && nlev < 1) return cudaErrorInvalidValue;  // flow_at reads at least one level
+  if (nlev > (arch == 426 ? 4 : 3)) return cudaErrorInvalidValue;  // front kernels are built for <= 3 (4.26: 4) levels
+  if (arch != 46 && feats == nullptr) return cudaErrorInvalidValue;
+  if (arch == 426 && blk > 0 && (prev_feat == nullptr || prev_s < 1)) return cudaErrorInvalidValue;
+  // arch 4.6 scale-2 front without a base plane whose levels are all at scale 4, 8, ...: the level taps are shared per cell
+  bool shared_taps = (arch == 46 && s == 2 && blk > 0 && base_f == nullptr);
   for (int j = 0; j < nlev; ++j) shared_taps = shared_taps && L.s[j] >= 4 && (L.s[j] & (L.s[j] - 1)) == 0;
-  const int nl = blk == 0 ? 0 : (nlev == 0 ? 1 : nlev);
-  if (op_type == OP_BF16)
-    launch_front_t<__nv_bfloat16>(nl, shared_taps, g, st, imgs_h, L, tasks, Hp, Wp, s, x_s2d);
-  else
-    launch_front_t<__half>(nl, shared_taps, g, st, imgs_h, L, tasks, Hp, Wp, s, x_s2d);
+  const bool bf16 = op_type == OP_BF16;
+  decltype(&launch_front_t<__half, 46>) go;
+  switch (arch) {
+    case 46: go = bf16 ? launch_front_t<__nv_bfloat16, 46> : launch_front_t<__half, 46>; break;
+    case 47: go = bf16 ? launch_front_t<__nv_bfloat16, 47> : launch_front_t<__half, 47>; break;
+    case 417: go = bf16 ? launch_front_t<__nv_bfloat16, 417> : launch_front_t<__half, 417>; break;
+    case 426: go = bf16 ? launch_front_t<__nv_bfloat16, 426> : launch_front_t<__half, 426>; break;
+    default: return cudaErrorInvalidValue;
+  }
+  go(nlev, shared_taps, g, st, imgs_h, feats, (const uint4*)prev_feat, prev_s, L, tasks, Hp, Wp, s, x_s2d);
   return cudaGetLastError();
 }
 
@@ -1480,41 +1056,19 @@ cudaError_t launch_final(const float4* imgs, const FlowState& fs, int lo, const 
 cudaError_t launch_front_up(int op_type, int arch, const uint2* imgs_h, const void* feats, const void* prev_feat, int prev_s,
                             int prev_k, const float4* F, const float* M, BatchTasks tasks, int Hp, int Wp, int k, void* x_s2d,
                             cudaStream_t st) {
-  if ((k != 2 && k != 4) || F == nullptr || M == nullptr || (arch != 46 && arch != 47 && arch != 417 && arch != 426))
-    return cudaErrorInvalidValue;
+  if ((k != 2 && k != 4) || F == nullptr || M == nullptr || (arch != 46 && feats == nullptr)) return cudaErrorInvalidValue;
+  if (arch == 426 && (prev_feat == nullptr || prev_s < 1 || prev_k < 1)) return cudaErrorInvalidValue;
   const dim3 g((unsigned)((Wp * k + 63) / 64), (unsigned)(Hp * k / 2), (unsigned)tasks.n);
-  if (arch == 426) {
-    if (feats == nullptr || prev_feat == nullptr || prev_s < 1 || prev_k < 1) return cudaErrorInvalidValue;
-    if (op_type == OP_BF16)
-      VFI_LAUNCH((front_up426_kernel<__nv_bfloat16>), g, 128, 0, st, imgs_h, (const uint2*)feats, (const uint4*)prev_feat, prev_s,
-                 prev_k, F, M, tasks, Hp, Wp, k, (__nv_bfloat16*)x_s2d);
-    else
-      VFI_LAUNCH((front_up426_kernel<__half>), g, 128, 0, st, imgs_h, (const uint2*)feats, (const uint4*)prev_feat, prev_s, prev_k,
-                 F, M, tasks, Hp, Wp, k, (__half*)x_s2d);
-    return cudaGetLastError();
+  const bool bf16 = op_type == OP_BF16;
+  decltype(&launch_front_up_t<__half, 46>) go;
+  switch (arch) {
+    case 46: go = bf16 ? launch_front_up_t<__nv_bfloat16, 46> : launch_front_up_t<__half, 46>; break;
+    case 47: go = bf16 ? launch_front_up_t<__nv_bfloat16, 47> : launch_front_up_t<__half, 47>; break;
+    case 417: go = bf16 ? launch_front_up_t<__nv_bfloat16, 417> : launch_front_up_t<__half, 417>; break;
+    case 426: go = bf16 ? launch_front_up_t<__nv_bfloat16, 426> : launch_front_up_t<__half, 426>; break;
+    default: return cudaErrorInvalidValue;
   }
-  if (arch == 417) {
-    if (feats == nullptr) return cudaErrorInvalidValue;
-    if (op_type == OP_BF16)
-      VFI_LAUNCH((front_up417_kernel<__nv_bfloat16>), g, 128, 0, st, imgs_h, (const uint4*)feats, F, M, tasks, Hp, Wp, k,
-                 (__nv_bfloat16*)x_s2d);
-    else
-      VFI_LAUNCH((front_up417_kernel<__half>), g, 128, 0, st, imgs_h, (const uint4*)feats, F, M, tasks, Hp, Wp, k, (__half*)x_s2d);
-    return cudaGetLastError();
-  }
-  if (arch == 47) {
-    if (feats == nullptr) return cudaErrorInvalidValue;
-    if (op_type == OP_BF16)
-      VFI_LAUNCH((front_up47_kernel<__nv_bfloat16>), g, 128, 0, st, imgs_h, (const uint2*)feats, F, M, tasks, Hp, Wp, k,
-                 (__nv_bfloat16*)x_s2d);
-    else
-      VFI_LAUNCH((front_up47_kernel<__half>), g, 128, 0, st, imgs_h, (const uint2*)feats, F, M, tasks, Hp, Wp, k, (__half*)x_s2d);
-    return cudaGetLastError();
-  }
-  if (op_type == OP_BF16)
-    VFI_LAUNCH((front_up_kernel<__nv_bfloat16>), g, 128, 0, st, imgs_h, F, M, tasks, Hp, Wp, k, (__nv_bfloat16*)x_s2d);
-  else
-    VFI_LAUNCH((front_up_kernel<__half>), g, 128, 0, st, imgs_h, F, M, tasks, Hp, Wp, k, (__half*)x_s2d);
+  go(g, st, imgs_h, feats, (const uint4*)prev_feat, prev_s, prev_k, F, M, tasks, Hp, Wp, k, x_s2d);
   return cudaGetLastError();
 }
 

@@ -550,7 +550,6 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
   const float4* imgs = (const float4*)c->imgs.p;
   const uint2* imgs_h = (const uint2*)c->imgs_h.p;
   const void* feats = c->arch != 46 ? c->feats.p : nullptr;
-  const int feat_ch = c->arch == 417 ? 8 : 4;
   const int nb = g.nb;
   float4* F = (float4*)c->flow.p;  // accumulated full-resolution flow / mask, written only by "dense" fronts
   float* M = (float*)c->mask.p;
@@ -579,13 +578,6 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
   auto span_end = [&]() {
     if (c->profile) cudaEventRecord(c->prof_spans.back().e1, st);
   };
-  // The last block's front stores the accumulated flow too and `final` adds one level to it.  VFI_FLOW_STORE_LAST=0: it
-  // does not, `final` adds the last TWO levels on the fly: the largest front then saves its 20 B/px store, but `final`
-  // reads a second level with eight taps per pixel, which makes it instruction bound - so storing stays the default.
-  static const bool store_last = [] {
-    const char* e = std::getenv("VFI_FLOW_STORE_LAST");
-    return !(e && e[0] == '0');
-  }();
   for (int i = 0; i < nb; ++i) {
     const int s = g.s[i];
     const int Hs = g.Hp * g.k[i] / s, Ws = g.Wp * g.k[i] / s;
@@ -605,14 +597,11 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
       LAUNCH(launch_front_up(c->op_type, c->arch, imgs_h, feats, pfeat, ps, g.k[i - 1], F, M, tasks, g.Hp, g.Wp, g.k[i], c->x.p,
                              st));
     } else if (i == 0 || i < dense) {
-      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, feat_ch, pfeat, ps, fs, i, 0, nullptr, nullptr, nullptr,
-                          nullptr, tasks, g.Hp, g.Wp, s, c->x.p, st));
-    } else if (i == nb - 1 && have_base && !store_last && i - lo + 1 <= 2) {
-      // last block: read the dense planes (+ the levels since), store nothing; `final` adds those levels and this one
-      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, feat_ch, pfeat, ps, fs, i, lo, F, M, nullptr, nullptr, tasks,
-                          g.Hp, g.Wp, s, c->x.p, st));
+      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, pfeat, ps, fs, i, 0, nullptr, nullptr, nullptr, nullptr,
+                          tasks, g.Hp, g.Wp, s, c->x.p, st));
     } else {
-      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, feat_ch, pfeat, ps, fs, i, lo, have_base ? F : nullptr,
+      // a dense front stores the accumulated flow, the last one too: `final` adding two levels per pixel is instruction bound
+      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, pfeat, ps, fs, i, lo, have_base ? F : nullptr,
                           have_base ? M : nullptr, F, M, tasks, g.Hp, g.Wp, s, c->x.p, st));
       have_base = true;
       lo = i;

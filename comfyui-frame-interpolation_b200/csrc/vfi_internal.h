@@ -135,10 +135,10 @@ cudaError_t launch_encode(const float4* imgs, const float* w0, const float* b0, 
                           float* e16, uint2* feats, int n, int Hp, int Wp, cudaStream_t st);
 cudaError_t launch_head0(int op_type, const float4* imgs, const float* w, const float* bias, void* out, int n, int Hp,
                          int Wp, cudaStream_t st);
-// feats: arch 4.7 half4 planes (feat_ch 4), arch 4.17 16-bit space-to-depth planes (feat_ch 8), arch 4.26 16-bit
-// space-to-depth planes of 4 channels (feat_ch 4, arch 426), or nullptr (4.6).  prev_feat: arch 4.26, blocks > 0: the
-// previous block's 8 lastconv feature channels [B, Hp/prev_s, Wp/prev_s, 8] 16-bit.
-cudaError_t launch_front(int op_type, int arch, const float4* imgs, const uint2* imgs_h, const void* feats, int feat_ch,
+// arch 46, 47, 417 or 426.  feats: arch 4.7 half4 planes, arch 4.17 / 4.26 16-bit space-to-depth planes of 8 / 4
+// channels, or nullptr (4.6).  prev_feat: arch 4.26, blocks > 0: the previous block's 8 lastconv feature channels
+// [B, Hp/prev_s, Wp/prev_s, 8] 16-bit.
+cudaError_t launch_front(int op_type, int arch, const float4* imgs, const uint2* imgs_h, const void* feats,
                          const void* prev_feat, int prev_s, const FlowState& fs, int blk, int lo,
                          const float4* base_f, const float* base_m, float4* out_f, float* out_m, BatchTasks tasks,
                          int Hp, int Wp, int s, void* x_s2d, cudaStream_t st);
