@@ -242,11 +242,10 @@ int build_conv_s2(vfi_ctx* c, TapConvLayer& L, int Cs, int creal, int cout, int 
   return VFI_OK;
 }
 
-// 3x3 taps over all `ch` input channels.  ring: k-block-major (kb, tap) entries of 64 channels each, the order the
-// ring pipeline consumes the window in (tapconv.cu); the packed weights follow the same order.
-void set_taps_3x3(TapConvLayer& L, int ch, bool ring) {
-  L.ring = ring ? 1 : 0;
-  const int nkb = ring ? ch / 64 : 1;
+// 3x3 taps over all `ch` input channels.  kb_major: k-block-major (kb, tap) entries of 64 channels each (ch % 64 == 0),
+// else one entry per tap over all channels; the packed weights follow the same order.
+void set_taps_3x3(TapConvLayer& L, int ch, bool kb_major) {
+  const int nkb = kb_major ? ch / 64 : 1;
   L.ntaps = 9 * nkb;
   for (int kb = 0; kb < nkb; ++kb)
     for (int e = 0; e < 9; ++e) {
@@ -254,21 +253,8 @@ void set_taps_3x3(TapConvLayer& L, int ch, bool ring) {
       t.dy = (int16_t)(e / 3 - 1);
       t.dx = (int16_t)(e % 3 - 1);
       t.chunk0 = (int16_t)(kb * 8);
-      t.nk16 = (int16_t)(ring ? 4 : ch / 16);
+      t.nk16 = (int16_t)(kb_major ? 4 : ch / 16);
     }
-}
-
-// Wide, deep layers (c = 128, 192; the ResConvs stream their weights instead): with the whole window staged
-// per tile the resident weight slice leaves room for only n_cta = 16 output channels, and every wgmma reads its whole
-// 64-row A block from shared memory whatever its N, so narrow CTAs re-read the window once per split.  The ring
-// pipeline stages one 64-channel k-block at a time, which frees shared memory for n_cta = 32 (c = 192) / 64 (c = 128).
-// VFI_RING=0 disables it (A/B runs).
-bool want_ring(int ch) {
-  static const bool on = [] {
-    const char* e = std::getenv("VFI_RING");
-    return !(e && e[0] == '0');
-  }();
-  return on && ch >= 128 && ch % 64 == 0;
 }
 
 int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const float* w, const float* bias) {
@@ -282,10 +268,9 @@ int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const 
   int real_taps = 9;
   if (ch >= 96) {
     // streamed weights (tapconv.cu): all channels per CTA up to the wgmma's N = 128, else two halves of 96.  The taps
-    // keep the K order of the resident-weight plans: k-block-major (the ring's) at c = 128 / 192, tap-major at c = 96.
+    // keep the K order of the resident-weight plans: k-block-major at c = 128 / 192, tap-major at c = 96.
     set_taps_3x3(L, ch, ch % 64 == 0);
     real_taps = L.ntaps;
-    L.ring = 0;
     L.wstream = 1;
     L.nsplit = ch > 128 ? 2 : 1;
     L.n_cta = ch / L.nsplit;
@@ -296,13 +281,12 @@ int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const 
       L.ktotal16 += t.nk16;
     }
   } else {
-    const bool ring = want_ring(ch);
-    set_taps_3x3(L, ch, ring);
-    choose_split(L, {1, 2, 3, 4, 6, 8, 12}, ring ? 2 : 3);
+    set_taps_3x3(L, ch, false);
+    choose_split(L, {1, 2, 3, 4, 6, 8, 12}, 3);
   }
   // (conv(x) + b) * beta + x  ==  conv_{w*beta}(x) + b*beta + x : beta is folded into the packed weights (one 16-bit
   // rounding of w*beta instead of w) so the epilogue is a pure add
-  auto wf = [&](int e, int ci, int n) -> float {  // e = kb * 9 + tap (kb = 0 unless ring), ci relative to the k-block
+  auto wf = [&](int e, int ci, int n) -> float {  // e = kb * 9 + tap (kb = 0 if tap-major), ci relative to the k-block
     if (e >= real_taps) return 0.f;
     const int tap = e % 9, cin = (e / 9) * 64 + ci;
     return w[(((size_t)n * ch + cin) * 3 + tap / 3) * 3 + tap % 3] * beta[n];
@@ -327,10 +311,12 @@ int build_lastconv(vfi_ctx* c, TapConvLayer& L, int ch, int cout, const float* w
   L.ktotal16 = 9 * (ch / 16);
   L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
   L.epi_mode = EPI_LASTCONV;
-  const bool ring = want_ring(ch);
-  set_taps_3x3(L, ch, ring);
-  choose_split(L, {1, 5}, 2);
-  if (ring && L.nsplit != 1) {  // the ring only pays when it keeps all 80 columns in one CTA (c = 128)
+  if (ch == 128) {  // streamed weights (tapconv.cu), all 80 columns in one CTA
+    set_taps_3x3(L, ch, true);
+    L.wstream = 1;
+    L.nsplit = 1;
+    L.n_cta = 80;
+  } else {
     set_taps_3x3(L, ch, false);
     choose_split(L, {1, 5}, 2);
   }
@@ -368,9 +354,15 @@ int build_lastfeat(vfi_ctx* c, TapConvLayer& L, int ch, int cout, const float* w
   L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
   L.epi_mode = EPI_BIAS;
   L.out_s2d = 2;
-  const bool ring = want_ring(ch);
-  set_taps_3x3(L, ch, ring);
-  choose_split(L, {2, 4, 8}, 2);
+  if (ch >= 128) {  // streamed weights (tapconv.cu), all 128 columns in one CTA
+    set_taps_3x3(L, ch, true);
+    L.wstream = 1;
+    L.nsplit = 1;
+    L.n_cta = 128;
+  } else {
+    set_taps_3x3(L, ch, false);
+    choose_split(L, {2, 4, 8}, 2);
+  }
   auto oc_of = [](int n) {
     const int f = n & 7, pos = n >> 3, py = pos >> 2, px = pos & 3;
     return 4 * (5 + f) + 2 * (py & 1) + (px & 1);

@@ -10,10 +10,10 @@
 // Why a second conv kernel: tapconv.cu keeps a layer's whole weight slice resident in shared memory (RIFE: <= 110 KB
 // per CTA).  FILM's layers have up to 9 x 2442 x 512 weights (22 MB), so here BOTH operands stream:
 //   A  the input window of a tile (tile + halo) for ONE 64-channel k-block, dropped into shared memory by TMA as rows of
-//      128 B (SWIZZLE_128B) - exactly tapconv's ring slot: every filter tap is a descriptor START ADDRESS into the
-//      window ((dy*halo_w + dx) * 128 B, 8-row-group stride SBO = halo_w * 128 B), a K=16 step a 32-byte shift.  One CTA
-//      pass covers mt = 2 tiles of 16 x 8 output pixels, one per MMA warpgroup, so a weight slice read from L2 feeds
-//      2 x 128 rows;
+//      128 B (SWIZZLE_128B) - the layout of one k-block of tapconv's staged window: every filter tap is a descriptor
+//      START ADDRESS into the window ((dy*halo_w + dx) * 128 B, 8-row-group stride SBO = halo_w * 128 B), a K=16 step a
+//      32-byte shift.  One CTA pass covers mt = 2 tiles of 16 x 8 output pixels, one per MMA warpgroup, so a weight
+//      slice read from L2 feeds 2 x 128 rows;
 //   B  the weights of one (k-block, tap): [n_cta rows][64 channels = 128 B, 16-byte chunks XOR (n & 7)] = the
 //      SWIZZLE_128B K-major B operand bit for bit, packed that way on the host, one cp.async.bulk per slot.
 // A layer may read its input channels from TWO tensors (k-blocks [0, nkb0) from source 0, the rest from source 1):
@@ -28,7 +28,6 @@
 // Pipelines: A ring (2-4 slots, full = TMA bytes, empty = both warpgroups after the k-block's last tap), B ring (3-8
 // slots, full = bulk-copy bytes, empty = both warpgroups after the tap's MMAs have completed).  Every wait is bounded
 // (ptx.cuh mbar_wait) and traps.
-#include <cstdlib>
 #include <cstring>
 #include <type_traits>
 
@@ -542,10 +541,6 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
   if (cps > p.npasses) cps = p.npasses;
   p.ctas_per_split = cps;
   const int grid = cps * p.nsplit;
-  static const bool pdl = [] {
-    const char* e = std::getenv("VFI_PDL");
-    return !(e && e[0] == '0');
-  }();
   auto go = [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
     if (e != cudaSuccess) return e;
@@ -555,14 +550,10 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
     cfg.dynamicSmemBytes = p.smem_bytes;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
-    int na = 0;
-    if (pdl) {
-      attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[na].val.programmaticStreamSerializationAllowed = 1;
-      ++na;
-    }
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, p);
   };
   auto pick_n = [&](auto tag, auto ext) -> cudaError_t {

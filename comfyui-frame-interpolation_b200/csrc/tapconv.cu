@@ -16,39 +16,38 @@
 // once (x1.41 halo), not 9x as with im2col.  Weights of the CTA's output-channel slice are resident in shared memory
 // for the whole launch (one bulk copy, already in the swizzled operand layout).
 //
-// Channel-major MMAs (p.cmajor, template CM: non-ring 3 x 3 convs over 64 input channels with n_cta = 64 and a staged
-// 16-bit NHWC output).  The
-// operand roles swap: the packed weights are byte for byte a K-major SWIZZLE_128B A operand (64 output-channel rows)
-// and the window a K-major B operand whose 8-row groups are the tile's 16 rows of 8 cells (SBO = halo_w * 128 B), so
-// ONE m64n128k16 per K=16 step computes the whole tile.  Per step shared memory then supplies 2 KB of weights + 4 KB of
-// window instead of 2 x (2 KB + 2 KB): with cells on M and N = 64 the two MMAs alone need all of an SM's shared-memory
-// bandwidth at the tensor peak (128 B/clk against 1/16 B per MAC), channel-major three quarters of it.  Same products
-// in the same K order into fp32: the outputs are bit-identical to the cell-major form (DESIGN.md section 5 has the
-// measured gain).
+// Channel-major MMAs (p.cmajor, template CM: 3 x 3 convs over 64 input channels with n_cta = 64 and a staged 16-bit
+// NHWC output).  The operand roles swap: the packed weights are byte for byte a K-major SWIZZLE_128B A operand (64
+// output-channel rows) and the window a K-major B operand whose 8-row groups are the tile's 16 rows of 8 cells (SBO =
+// halo_w * 128 B), so ONE m64n128k16 per K=16 step computes the whole tile.  Per step shared memory then supplies 2 KB
+// of weights + 4 KB of window instead of 2 x (2 KB + 2 KB): with cells on M and N = 64 the two MMAs alone need all of
+// an SM's shared-memory bandwidth at the tensor peak (128 B/clk against 1/16 B per MAC), channel-major three quarters
+// of it.  Same products in the same K order into fp32: the outputs are bit-identical to the cell-major form (DESIGN.md
+// section 5 has the measured gain).
 //
-// Streamed weights (p.wstream, template WS: the wide ResConvs, c = 96 / 128 / 192).  A resident weight slice of such a
-// layer leaves room for only 48 - 64 output channels per CTA, so every tile's window was read from L2 and shared memory
-// once per output-channel split (2 - 4 times), and the narrow wgmma N left the tensor cores waiting on shared memory
-// (an SS wgmma reads its 2 KB A block whatever its N).  Here the window of a tile is staged once with all its k-blocks
-// and held until the epilogue, and the weights stream through a ring of slots of four K=16 steps each (the packed
-// [K16 / 4][n_cta][128 B] rows, one bulk copy per slot) fed by a second producer warp: n_cta = 96 / 128 / 96 output
-// channels per CTA.  Both MMA warpgroups take a tile each and consume every slot in step, so one weight fill from L2
-// feeds 256 cells.  The K=16 steps keep the order of the layer's tap list (k-block-major at c = 128 / 192 as the ring
-// plan issued them, tap-major at c = 96, whose two extra zero-weight steps only complete the last slot): every output
-// is the same fp32 sum in the same order as with resident weights.
+// Streamed weights (p.wstream, template WS: the wide ResConvs, c = 96 / 128 / 192, block 1's lastconv, c = 128, and
+// the 4.26 feature conv at c = 128 / 192).  A resident weight slice of such a layer leaves room for only 16 - 64
+// output channels per CTA, so every tile's window would be read from L2 and shared memory once per output-channel
+// split, and the narrow wgmma N leaves the tensor cores waiting on shared memory (an SS wgmma reads its 2 KB A block
+// whatever its N).  Here the window of a tile is staged once with all its k-blocks and held until the epilogue, and the
+// weights stream through a ring of slots of four K=16 steps each (the packed [K16 / 4][n_cta][128 B] rows, one bulk
+// copy per slot) fed by a second producer warp: n_cta = 96 / 128 / 96 output channels per CTA for the ResConvs, all
+// 80 / 128 columns for lastconv / the feature conv.  Both MMA warpgroups take a tile each and consume every slot in
+// step, so one weight fill from L2 feeds 256 cells.  The K=16 steps keep the order of the layer's tap list (k-block-major at c = 128 / 192,
+// tap-major at c = 96, whose two extra zero-weight steps only complete the last slot): every output is the same fp32
+// sum in the same order as with resident weights.
 //
 // Warp roles (288 threads, 1 CTA/SM, persistent over tiles; WS: 320):
 //   warpgroups 0, 1 : MMA + epilogue.  Warpgroup w takes the CTA's tiles w, w + 2, ... and keeps the whole tile's
 //                     accumulators (2 x 64 rows x n_cta columns, fp32) in registers, so one warpgroup's epilogue
-//                     overlaps the other's MMAs: +shift (held in registers for the launch), +residual (non-ring
-//                     ResConv: ldmatrix from the tile's still-held window stage, then the stage is released; ring
-//                     layers: from global memory), LeakyReLU, 16-bit; NHWC outputs are stmatrix'ed into a swizzled
-//                     per-warpgroup staging tile and leave as TMA tensor stores (one thread, clipped at the image
-//                     border); lastconv writes whole float4 flow texels, the space-to-depth forms direct stores.
+//                     overlaps the other's MMAs: +shift (held in registers for the launch), +residual (ResConv:
+//                     ldmatrix from the tile's still-held window stage, then the stage is released), LeakyReLU,
+//                     16-bit; NHWC outputs are stmatrix'ed into a swizzled per-warpgroup staging tile and leave as TMA
+//                     tensor stores (one thread, clipped at the image border); lastconv writes whole float4 flow
+//                     texels, the space-to-depth forms direct stores.
 //   warp 8          : one elected lane: weight bulk copy, then one 4-D TMA tensor copy per k-block and tile
 //   warp 9 (WS)     : one elected lane: one bulk copy per weight slot, the whole weight stream once per pair of tiles
 #include <algorithm>
-#include <cstdlib>
 #include <type_traits>
 
 #include "ptx.cuh"
@@ -58,7 +57,7 @@ namespace vfi {
 
 namespace {
 
-constexpr int kMaxStages = 6;   // window stages or ring slots
+constexpr int kMaxStages = 6;   // window stages
 constexpr int kMaxWSlots = 8;   // streamed weight slots
 struct Ctrl {
   uint64_t w_full;
@@ -138,7 +137,7 @@ struct TileIter {
 // warpgroup.arrive instead of injecting an arrive in front of every MMA and ending each one's scoreboard group.
 template <int N, bool CM, typename T>
 __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc)[2][N / 2], uint32_t a_base,
-                                             uint32_t b_base, uint32_t accumulate_first) {
+                                             uint32_t b_base) {
   if constexpr (CM) {
 #pragma unroll
     for (int r = 0; r < kCmRuns; ++r) {
@@ -147,7 +146,7 @@ __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc
       const uint64_t x64 = ((uint64_t)d.y << 32) | (uint64_t)(a_base + d.x);
 #pragma unroll
       for (int i = 0; i < kCmRunLen; ++i)
-        wgmma_ss<128, T>(&acc[0][0], w64 + 2u * i, x64 + 2u * i, (r | i) ? 1u : accumulate_first);
+        wgmma_ss<128, T>(&acc[0][0], w64 + 2u * i, x64 + 2u * i, (r | i) ? 1u : 0u);
     }
     return;
   }
@@ -161,7 +160,7 @@ __device__ __forceinline__ void issue_window(const TapConvParams& p, float (&acc
       uint64_t b64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b_base + d.z);
 #pragma unroll 1
       for (int i = 0; i < p.run_len; ++i) {
-        wgmma_ss<N, T>(acc[h], a64, b64, (r | i) ? 1u : accumulate_first);
+        wgmma_ss<N, T>(acc[h], a64, b64, (r | i) ? 1u : 0u);
         a64 += 2;
         b64 += 2;
       }
@@ -188,10 +187,10 @@ __device__ __forceinline__ void issue_wslot(const TapConvParams& p, float (&acc)
   }
 }
 
-template <typename T, bool RING, bool LAST, int N, bool CM, bool WS>
+template <typename T, bool LAST, int N, bool CM, bool WS>
 __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(const __grid_constant__ TapConvParams p) {
-  static_assert(!CM || (N == 64 && !RING && !LAST), "channel-major: 64 output channels, staged window, 16-bit output");
-  static_assert(!WS || (!CM && !RING && !LAST), "streamed weights: cells on M, staged window, 16-bit output");
+  static_assert(!CM || (N == 64 && !LAST), "channel-major: 64 output channels, 16-bit output");
+  static_assert(!WS || !CM, "streamed weights: cells on M");
   extern __shared__ __align__(1024) uint8_t smem[];
   // Programmatic dependent launch (launch_tapconv sets the attribute): the next kernel in the stream may start its
   // CTAs as soon as every CTA of this grid has passed this point, i.e. while our last tiles are still running - they do
@@ -268,33 +267,20 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
       // weights do not depend on the previous kernel; its output (our input tensor) does
       asm volatile("griddepcontrol.wait;" ::: "memory");
       TileIter it(p, first, tstep);
-      uint32_t stage = 0, eph = 1;  // window stage / ring slot and the parity of its "empty" barrier
+      uint32_t stage = 0, eph = 1;  // window stage and the parity of its "empty" barrier
       for (int k = 0; k < my_tiles; ++k, it.next()) {
         const int gy0 = it.ty * kTileH + p.halo_y0, gx0 = it.tx * kTileW + p.halo_x0;
-        if (RING) {
-          for (int kb = 0; kb < p.nkb; ++kb) {
-            const uint32_t full = bar_afull + 16 * stage + 8 * (k & 1);  // tile k goes to warpgroup k % 2
-            mbar_wait(bar_aempty + 8 * stage, eph);
-            mbar_arrive_expect_tx(full, p.tx_bytes);
-            tma_load_4d(a_smem + stage * p.stage_bytes, &p.tm64, full, kb * 64, gx0, gy0, it.b);
-            if (++stage == (uint32_t)S) {
-              stage = 0;
-              eph ^= 1u;
-            }
-          }
-        } else {
-          const uint32_t full = bar_afull + 16 * stage + 8 * (k & 1);
-          mbar_wait(bar_aempty + 8 * stage, eph);
-          mbar_arrive_expect_tx(full, p.tx_bytes);
-          const uint32_t dst = a_smem + stage * p.stage_bytes;
-          for (int kb = 0; kb < p.nkb; ++kb) {
-            const bool tail = has_tail && (kb == p.nkb - 1);
-            tma_load_4d(dst + p.kb_off[kb], tail ? &p.tm32 : &p.tm64, full, kb * 64, gx0, gy0, it.b);
-          }
-          if (++stage == (uint32_t)S) {
-            stage = 0;
-            eph ^= 1u;
-          }
+        const uint32_t full = bar_afull + 16 * stage + 8 * (k & 1);  // tile k goes to warpgroup k % 2
+        mbar_wait(bar_aempty + 8 * stage, eph);
+        mbar_arrive_expect_tx(full, p.tx_bytes);
+        const uint32_t dst = a_smem + stage * p.stage_bytes;
+        for (int kb = 0; kb < p.nkb; ++kb) {
+          const bool tail = has_tail && (kb == p.nkb - 1);
+          tma_load_4d(dst + p.kb_off[kb], tail ? &p.tm32 : &p.tm64, full, kb * 64, gx0, gy0, it.b);
+        }
+        if (++stage == (uint32_t)S) {
+          stage = 0;
+          eph ^= 1u;
         }
       }
     }
@@ -319,16 +305,14 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
 #pragma unroll
     for (int j = 0; j < N / 8; ++j) sh[j] = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + c2));
   }
-  // the previous kernel may still be reading the buffer we store to (ping-pong) and ring ResConv layers read the
-  // residual from global memory: every storing / loading thread orders itself after the previous grid
+  // the previous kernel may still be reading the buffer we store to (ping-pong): every storing thread orders itself
+  // after the previous grid
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (!WS) mbar_wait(bar_w, 0);
   const uint32_t a_lo0 = (1u << 16) | (a_smem >> 4);  // LBO(=1) | start address, 16-byte units
   const uint32_t b_lo0 = (1u << 16) | (w_smem >> 4);
-  const uint32_t per_tile = RING ? (uint32_t)p.nkb : 1u;  // stages / slots one tile consumes
-  const uint32_t b_kb = (9u * (uint32_t)p.n_cta * 128u) >> 4;  // ring: weight bytes of one k-block, 16-byte units
   const uint32_t stage_units = p.stage_bytes >> 4;
-  uint32_t stage = 0, ph_bits = 0;  // window stage / ring slot; bit s: parity of this warpgroup's next wait on stage s
+  uint32_t stage = 0, ph_bits = 0;  // window stage; bit s: parity of this warpgroup's next wait on stage s
   auto advance = [&](uint32_t n) {
     stage += n;
     while (stage >= (uint32_t)S) stage -= (uint32_t)S;
@@ -337,7 +321,7 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
     mbar_wait(bar_afull + 16 * stage + 8 * (uint32_t)g, (ph_bits >> stage) & 1u);
     ph_bits ^= 1u << stage;
   };
-  advance((uint32_t)g * per_tile);
+  advance((uint32_t)g);
   const float slope = (p.epi_mode == EPI_BIAS) ? 1.f : 0.2f;  // max(a, slope * a): LeakyReLU(0.2), or no activation
   // TMA-stored outputs: each warpgroup packs its tile into its own staging tile, [box][16 x 8 pixels][kBoxC channels]
   // swizzled like the box rows, and one thread stores it as N / kBoxC tensor boxes
@@ -379,29 +363,10 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_wsempty + 8 * prev);
       if (!residual && lane == 0) mbar_arrive(bar_aempty + 8 * stage);
-    } else if (RING) {
-      uint32_t prev = 0;
-      for (int kb = 0; kb < p.nkb; ++kb) {
-        wait_full();
-        wgmma_fence();
-        issue_window<N, CM, T>(p, acc, a_lo0 + stage * stage_units, b_lo0 + (uint32_t)kb * b_kb, kb > 0 ? 1u : 0u);
-        wgmma_commit();
-        if (kb > 0) {  // the previous slot's MMAs have read it
-          wgmma_wait<1>();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_aempty + 8 * prev);
-        }
-        prev = stage;
-        advance(1u);
-      }
-      wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_aempty + 8 * prev);
-      advance(per_tile);  // the other warpgroup's tile
     } else {
       wait_full();
       wgmma_fence();
-      issue_window<N, CM, T>(p, acc, a_lo0 + stage * stage_units, b_lo0, 0u);
+      issue_window<N, CM, T>(p, acc, a_lo0 + stage * stage_units, b_lo0);
       wgmma_commit();
       wgmma_wait<0>();
       if (!residual) {  // window free once the MMAs have read it (ResConv reads its residual from it first)
@@ -442,7 +407,7 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
           acc[h][4 * j + 3] += s.y;
         }
     }
-    if (residual && !RING) {
+    if (residual) {
       // the residual is the centre of the tile's staged window, still held: channel n of window pixel
       // (y - halo_y0, x - halo_x0), read as 8 x 8 (pixel, channel) matrices straight into the accumulator layout
       const uint32_t win = a_smem + stage * p.stage_bytes;
@@ -497,23 +462,7 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_aempty + 8 * stage);
     }
-    if (residual && RING) {  // ring slots are recycled before the epilogue: the residual comes from global memory
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int gy = gy0 + 8 * h + 2 * wq + e, gx = gx0 + px;
-          if (gy >= p.H || gx >= p.W) continue;
-          const T* rrow = reinterpret_cast<const T*>(p.in) + (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.cin + n0 + c2;
-#pragma unroll
-          for (int j = 0; j < N / 8; ++j) {
-            const float2 rf = Pack2<T>::unpack(__ldg(reinterpret_cast<const unsigned int*>(rrow + 8 * j)));
-            acc[h][4 * j + 2 * e] += rf.x;
-            acc[h][4 * j + 2 * e + 1] += rf.y;
-          }
-        }
-    }
-    if (!RING) advance((uint32_t)kMmaGroups);
+    advance((uint32_t)kMmaGroups);
 
     if (tma_out) {
       if (leader) bulk_wait_read<0>();  // the previous tile's stores have read the staging tile
@@ -765,38 +714,26 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
   p.w_bytes = (uint32_t)((L.ktotal16 + 3) / 4) * (uint32_t)L.n_cta * 128u;
   // input window: one 1024-aligned region per k-block (64 channels = 128-byte rows; 32-channel tail = 64-byte rows)
   p.nkb = (L.cin + 63) / 64;
-  p.ring = L.ring;
   p.wstream = L.wstream;
   if (L.ktotal16 > kMaxK16) return 0;
   // n_cta = the wgmma N: whole 8-row swizzle atoms of B, and a multiple of 16 with an instantiated kernel (<= 96: two
   // 64-row accumulators of n_cta fp32 columns per thread)
   // (streamed weights, whose shift is read per tile instead: up to 128)
   if (p.nkb > kMaxKBlocks || L.n_cta > (L.wstream ? 128 : 96) || (L.n_cta & 15) || L.n_cta < 16) return 0;
-  if (L.ring && ((L.cin & 63) || L.ntaps != 9 * p.nkb || L.ktotal16 != 36 * p.nkb)) return 0;
-  if (L.wstream && (L.ring || L.epi_mode == EPI_LASTCONV || L.out_s2d != 0 || (L.ktotal16 & 3))) return 0;
+  if (L.wstream && (L.ktotal16 & 3)) return 0;
   uint32_t off = 0;
   p.tx_bytes = 0;
-  if (L.ring) {
-    // ring: every slot holds ONE k-block of a tile's window; p.stage_bytes / p.tx_bytes are per slot
-    const uint32_t bytes = (uint32_t)L.halo_w * (uint32_t)L.halo_h * 128u;
-    for (int kb = 0; kb < p.nkb; ++kb) p.kb_off[kb] = 0;
-    off = align_up(bytes, 1024);
-    p.tx_bytes = bytes;
-  } else {
-    for (int kb = 0; kb < p.nkb; ++kb) {
-      const bool tail = (kb == p.nkb - 1) && (L.cin & 63);
-      const uint32_t bytes = (uint32_t)L.halo_w * (uint32_t)L.halo_h * (tail ? 64u : 128u);
-      p.kb_off[kb] = off;
-      off += align_up(bytes, 1024);
-      p.tx_bytes += bytes;
-    }
+  for (int kb = 0; kb < p.nkb; ++kb) {
+    const bool tail = (kb == p.nkb - 1) && (L.cin & 63);
+    const uint32_t bytes = (uint32_t)L.halo_w * (uint32_t)L.halo_h * (tail ? 64u : 128u);
+    p.kb_off[kb] = off;
+    off += align_up(bytes, 1024);
+    p.tx_bytes += bytes;
   }
   p.stage_bytes = off;
   {
     // wgmma descriptor words per K=16 step (ptx.cuh): start>>4 [0,14) | LBO [16,30) ; SBO>>4 [32,46) | layout [62,64)
     // (1 = SWIZZLE_128B, 2 = SWIZZLE_64B); base_offset stays 0.
-    // Ring layers list their taps k-block-major, so entries [0,36) (k-block 0) serve every k-block: the kernel adds
-    // the slot address to A and kb * (9 * n_cta * 128 B) to B.
     uint4 step[kMaxK16];
     int j = 0;
     for (int e = 0; e < L.ntaps; ++e)
@@ -814,12 +751,11 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
       }
     // group the steps into runs of run_len = 4, 2 or 1 whose descriptors advance by 32 B (2 units) per step
     // (streamed weights: one entry per step, issue_wslot)
-    const int nsteps = L.ring ? 36 : L.ktotal16;  // ring: the first k-block's entries serve every slot
     int run_len = 1;
     for (int len : {4, 2}) {
       if (L.wstream) break;
-      bool ok = (nsteps % len) == 0;
-      for (int r = 0; ok && r < nsteps; r += len)
+      bool ok = (L.ktotal16 % len) == 0;
+      for (int r = 0; ok && r < L.ktotal16; r += len)
         for (int i = 1; i < len; ++i)
           ok = ok && step[r + i].x == step[r].x + 2u * i && step[r + i].y == step[r].y &&
                step[r + i].z == step[r].z + 2u * i;
@@ -829,17 +765,19 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
       }
     }
     p.run_len = run_len;
-    p.nruns = nsteps / run_len;
+    p.nruns = L.ktotal16 / run_len;
     for (int r = 0; r < p.nruns; ++r) p.mma[r] = step[r * run_len];
   }
   p.b_hi = (1024u >> 4) | kDescSw128;  // B: SBO = 8 rows x 128 B, SWIZZLE_128B
   p.off_w = align_up(kCtrlBytes, 1024);
   // 16-bit NHWC outputs leave through TMA tensor stores from one staging tile per MMA warpgroup (128 cells x n_cta
   // channels, 1024-aligned store boxes).  A dedicated region rather than the consumed window stage: the stage is free
-  // for the next fill as soon as the residual is read, and ring slots are recycled before the epilogue runs.  The
-  // staging costs window stages; a layer left with fewer than kMinStagedStages keeps direct stores (on H100 at 1080p
-  // the c = 128 ring ResConv with 2 slots instead of 3 and conv0.1 at c = 96 / 192 lost more than the stores gained).
+  // for the next fill as soon as the residual is read.  The staging costs window stages; a resident-weight layer left
+  // with fewer than kMinStagedStages keeps direct stores (on H100 at 1080p conv0.1 at c = 96 / 192 lost more than the
+  // stores gained).  lastconv's fp32 planes and the space-to-depth / patch forms always store directly.
   constexpr int kMinStagedStages = 3;
+  const uint32_t staged_out =
+      (L.epi_mode != EPI_LASTCONV && L.out_s2d == 0) ? (uint32_t)(kTileH * kTileW) * L.n_cta * 2u : 0u;
   auto fit = [&](uint32_t out_stage) {
     p.out_stage_bytes = out_stage;
     p.off_out = align_up(p.off_w + p.w_bytes, 1024);
@@ -857,7 +795,7 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
     // their epilogues at once, the tensor cores idle meanwhile), then 4 window stages (the next pass's windows load
     // during this one) down to the 2 the two tiles of a pass need, each with at least 3 weight slots in flight
     constexpr int kMinWSlots = 3;
-    for (uint32_t out_stage : {(uint32_t)(kTileH * kTileW) * L.n_cta * 2u, 0u})
+    for (uint32_t out_stage : {staged_out, 0u})
       for (int s = 4; s >= 2 && p.w_slots == 0; --s) {
         const uint32_t fixed = align_up(kCtrlBytes, 1024) + kMmaGroups * out_stage + (uint32_t)s * p.stage_bytes;
         if (fixed >= (uint32_t)kSmemLimit) continue;
@@ -875,19 +813,14 @@ int tapconv_plan(const TapConvLayer& L, TapConvParams* pp) {
     p.cmajor = 0;
     return stages;
   }
-  if (L.epi_mode != EPI_LASTCONV && L.out_s2d == 0) stages = fit((uint32_t)(kTileH * kTileW) * L.n_cta * 2u);
+  if (staged_out) stages = fit(staged_out);
   if (stages < kMinStagedStages) stages = fit(0u);
   p.stages = stages;
   p.smem_bytes = p.off_a + (uint32_t)stages * p.stage_bytes;  // stage sizes are multiples of 1024
   // Channel-major MMAs (top of this file) need exactly 64 output channels for the M of one wgmma, the whole window
   // held until the epilogue (its residual read) and the staging tile the transposed fragments are stored through.  The
-  // shared-memory plan is the same in both orientations.  VFI_TAPCONV_CMAJOR=0 keeps cells on M (A/B runs).
-  static const bool cmajor_on = [] {
-    const char* e = std::getenv("VFI_TAPCONV_CMAJOR");
-    return !(e && e[0] == '0');
-  }();
-  p.cmajor = (cmajor_on && !L.ring && L.n_cta == 64 && p.out_stage_bytes != 0 && p.nruns == kCmRuns &&
-              p.run_len == kCmRunLen) ? 1 : 0;
+  // shared-memory plan is the same in both orientations.
+  p.cmajor = (L.n_cta == 64 && p.out_stage_bytes != 0 && p.nruns == kCmRuns && p.run_len == kCmRunLen) ? 1 : 0;
   return stages;
 }
 
@@ -957,10 +890,6 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
   p.ctas_per_split = cps;
   const int grid = cps * L.nsplit;
   cudaError_t err;  // (per device: set on every launch, it is a cheap driver call)
-  static const bool pdl = [] {  // VFI_PDL=0: plain stream-ordered launches (A/B runs)
-    const char* e = std::getenv("VFI_PDL");
-    return !(e && e[0] == '0');
-  }();
   auto go = [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
     if (e != cudaSuccess) return e;
@@ -970,43 +899,39 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
     cfg.dynamicSmemBytes = p.smem_bytes;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
-    int na = 0;
-    if (pdl) {
-      attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[na].val.programmaticStreamSerializationAllowed = 1;
-      ++na;
-    }
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, p);
   };
-  const bool last = (L.epi_mode == EPI_LASTCONV);
-  auto pick_n = [&](auto tag, auto ring, auto lst) -> cudaError_t {
+  auto pick_n = [&](auto tag, auto lst) -> cudaError_t {
     using T = decltype(tag);
-    constexpr bool R = decltype(ring)::value, LA = decltype(lst)::value;
-    if constexpr (!R && !LA) {
-      if (p.cmajor) return go(tapconv_kernel<T, false, false, 64, true, false>);  // (tapconv_plan: n_cta == 64)
-      if (p.wstream) {  // the wide ResConvs: n_cta = 96 (c = 96, 192) or 128 (c = 128)
-        if (L.n_cta == 96) return go(tapconv_kernel<T, false, false, 96, false, true>);
-        if (L.n_cta == 128) return go(tapconv_kernel<T, false, false, 128, false, true>);
-        set_error("tapconv: streamed weights are instantiated for n_cta = 96 and 128 only");
-        return cudaErrorInvalidConfiguration;
+    constexpr bool LA = decltype(lst)::value;
+    if (p.wstream) {
+      // n_cta = 96 (ResConv c = 96, 192) or 128 (ResConv c = 128, the 4.26 feature conv); lastconv: all 80 columns
+      if constexpr (LA) {
+        if (L.n_cta == 80) return go(tapconv_kernel<T, true, 80, false, true>);
+      } else {
+        if (L.n_cta == 96) return go(tapconv_kernel<T, false, 96, false, true>);
+        if (L.n_cta == 128) return go(tapconv_kernel<T, false, 128, false, true>);
       }
+      set_error("tapconv: streamed weights are instantiated for n_cta = 96 and 128 (lastconv: 80) only");
+      return cudaErrorInvalidConfiguration;
     }
+    if constexpr (!LA)
+      if (p.cmajor) return go(tapconv_kernel<T, false, 64, true, false>);  // (tapconv_plan: n_cta == 64)
     switch (L.n_cta) {  // tapconv_plan admits multiples of 16 up to 96
-      case 16: return go(tapconv_kernel<T, R, LA, 16, false, false>);
-      case 32: return go(tapconv_kernel<T, R, LA, 32, false, false>);
-      case 48: return go(tapconv_kernel<T, R, LA, 48, false, false>);
-      case 64: return go(tapconv_kernel<T, R, LA, 64, false, false>);
-      case 80: return go(tapconv_kernel<T, R, LA, 80, false, false>);
-      default: return go(tapconv_kernel<T, R, LA, 96, false, false>);
+      case 16: return go(tapconv_kernel<T, LA, 16, false, false>);
+      case 32: return go(tapconv_kernel<T, LA, 32, false, false>);
+      case 48: return go(tapconv_kernel<T, LA, 48, false, false>);
+      case 64: return go(tapconv_kernel<T, LA, 64, false, false>);
+      case 80: return go(tapconv_kernel<T, LA, 80, false, false>);
+      default: return go(tapconv_kernel<T, LA, 96, false, false>);
     }
   };
   auto pick = [&](auto tag) -> cudaError_t {
-    using F = std::false_type;
-    using Tr = std::true_type;
-    if (L.ring) return last ? pick_n(tag, Tr{}, Tr{}) : pick_n(tag, Tr{}, F{});
-    return last ? pick_n(tag, F{}, Tr{}) : pick_n(tag, F{}, F{});
+    return L.epi_mode == EPI_LASTCONV ? pick_n(tag, std::true_type{}) : pick_n(tag, std::false_type{});
   };
   err = (op_type == OP_BF16) ? pick(__nv_bfloat16{}) : pick(__half{});
   if (err != cudaSuccess) return err;

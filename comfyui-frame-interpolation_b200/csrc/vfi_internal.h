@@ -40,7 +40,7 @@ struct TapEntry {
   int16_t nk16;     // number of K=16 MMA steps (16 input channels each)
 };
 
-constexpr int kMaxTaps = 27;  // 9 taps, or 9 taps x 3 k-blocks in k-block-major (ring) order
+constexpr int kMaxTaps = 27;  // 9 taps, or 9 taps x 3 k-blocks in k-block-major order
 constexpr int kTileH = 16, kTileW = 8;        // one CTA tile = 128 grid cells = two m64 wgmma row blocks
 constexpr int kSmemLimit = 232448;            // 227 KB opt-in maximum per CTA on sm_90
 
@@ -65,7 +65,6 @@ struct alignas(64) TapConvParams {
   int stages;
   int epi_mode, out_s2d;
   int nruns, run_len;    // MMA issue: nruns runs of run_len consecutive K=16 steps (mma[r] = first step of run r)
-  int ring;              // 1: the window streams through a ring of single k-block slots (see tapconv.cu)
   int cmajor;            // 1: channel-major MMAs, the 64 output channels on the wgmma M and the tile's 128 cells on N
   int wstream;           // 1: the weights stream through w_slots slots of four K=16 steps (see tapconv.cu)
   int w_slots, w_groups; //    slots in shared memory / slots per tile (ceil(K16 / 4))
@@ -91,8 +90,8 @@ struct TapConvLayer {
   int ntaps = 0, ktotal16 = 0;
   int halo_y0 = 0, halo_x0 = 0, halo_h = 0, halo_w = 0;
   int epi_mode = 0, out_s2d = 0;
-  int ring = 0;           // taps are listed k-block-major (kb, tap) with nk16 = 4; needs cin % 64 == 0
-  int wstream = 0;        // streamed weights, whole window per tile (ResConv, n_cta 96 / 128; see tapconv.cu)
+  int wstream = 0;        // streamed weights, whole window per tile (the ResConvs of blocks 0-2, block 1's lastconv
+                          // and the 4.26 feature conv of blocks 0 and 1; see tapconv.cu)
   TapEntry taps[kMaxTaps];
   void* w = nullptr;      // device
   float* shift = nullptr; // device

@@ -134,8 +134,8 @@ def test_resconv(engines, block, dtype, impl):
 
 @pytest.mark.parametrize("block", [3, 1, 0])
 def test_resconv_many_tiles(engines, block):
-    """More tiles than persistent CTAs: every CTA walks several tiles, so the window stages / ring slots, both MMA warpgroups'
-    tiles and all mbarrier phases wrap several times (blocks 0 and 1 run the k-block ring pipeline)."""
+    """More tiles than persistent CTAs: every CTA walks several tiles, so the window stages, both MMA warpgroups' tiles
+    and all mbarrier phases wrap several times (blocks 0 and 1 stream their weights: the weight slots wrap too)."""
     sd, e = engines
     eng, c = e["float16"], BLOCK_C[block]
     g = torch.Generator().manual_seed(40 + block)

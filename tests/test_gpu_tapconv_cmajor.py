@@ -71,8 +71,8 @@ def _max_abs(a, b):
 
 
 def test_plan_selects_block3_conv01_and_resconvs(engines):
-    """Channel-major runs exactly where the plan allows it: non-ring 3 x 3 convs over 64 input channels with 64 output
-    channels per CTA and a staged 16-bit NHWC output.  For RIFE 4.6 those are block 3's ResConvs, nothing else."""
+    """Channel-major runs exactly where the plan allows it: resident-weight 3 x 3 convs over 64 input channels with 64
+    output channels per CTA and a staged 16-bit NHWC output.  For RIFE 4.6 those are block 3's ResConvs, nothing else."""
     eng = engines["float16"]
     for b in range(4):
         for l in range(11):

@@ -334,6 +334,35 @@ def test_rife_flow_state_on_host(emu, sf):
     assert (mask - want_m).abs().max().item() <= 0.05
 
 
+@pytest.mark.parametrize("operand", ["float16", "bfloat16"])
+@pytest.mark.parametrize("arch", ["4.6", "4.26"])
+def test_streamed_weight_plans_on_host(emu, arch, operand):
+    """vfi_rife46_layer_plan of the loaded library: exactly the layers test_gpu_tapconv_wstream.py expects stream their
+    weights (blocks 0-2's ResConvs, block 1's lastconv, 4.26's feature conv of blocks 0 and 1), with their split, and fit
+    in shared memory."""
+    from test_gpu_tapconv_wstream import check_plan
+    sd = O.synthetic_state_dict(17, arch=arch)
+    names, code = _engine_names(arch)
+    hold = [sd[n].contiguous().float() for n in names]
+    ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+    numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+    ctx = C.c_void_p()
+    assert emu.vfi_create(0, C.byref(ctx)) == 0, emu.vfi_last_error()
+    assert emu.vfi_rife_load(ctx, code, ptrs, numel, len(hold), 0 if operand == "float16" else 1) == 0, emu.vfi_last_error()
+
+    def plan(block, layer):
+        st, nc, ns, sm, cm, ws, mc = C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int64()
+        assert emu.vfi_rife46_layer_plan(ctx, block, layer, C.byref(st), C.byref(nc), C.byref(ns), C.byref(sm),
+                                         C.byref(mc), C.byref(cm), C.byref(ws)) == 0, emu.vfi_last_error()
+        return dict(stages=st.value, n_cta=nc.value, nsplit=ns.value, smem_bytes=sm.value, cmajor=bool(cm.value),
+                    wstream=bool(ws.value))
+
+    try:
+        check_plan(plan, arch)
+    finally:
+        assert emu.vfi_destroy(ctx) == 0
+
+
 def test_load_refuses_a_wrong_checkpoint(emu):
     sd = O.synthetic_state_dict(0, 1.0)
     names, code = _engine_names("4.6")
