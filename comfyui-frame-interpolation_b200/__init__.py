@@ -1,4 +1,4 @@
-"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
+"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR, IFRNet) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
 
 Exports the same mapping names ComfyUI discovers in the reference's root __init__.py:23-47.
 """
@@ -7,6 +7,7 @@ from .film_node import FILM_VFI  # noqa: F401
 from .sepconv_node import SepconvVFI  # noqa: F401
 from .gmfss_node import GMFSS_Fortuna_VFI  # noqa: F401
 from .flavr_node import FLAVR_VFI  # noqa: F401
+from .ifrnet_node import IFRNet_VFI  # noqa: F401
 
 NODE_CLASS_MAPPINGS = {
     "RIFE VFI": RIFE_VFI,
@@ -14,6 +15,7 @@ NODE_CLASS_MAPPINGS = {
     "Sepconv VFI": SepconvVFI,
     "GMFSS Fortuna VFI": GMFSS_Fortuna_VFI,
     "FLAVR VFI": FLAVR_VFI,
+    "IFRNet VFI": IFRNet_VFI,
     "Make Interpolation State List": MakeInterpolationStateList,
     "VFI FloatToInt": FloatToInt,
 }
@@ -24,4 +26,5 @@ NODE_DISPLAY_NAME_MAPPINGS = {
     "Sepconv VFI": "Sepconv VFI (H100 native)",
     "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native)",
     "FLAVR VFI": "FLAVR VFI (H100 native)",
+    "IFRNet VFI": "IFRNet VFI (H100 native)",
 }

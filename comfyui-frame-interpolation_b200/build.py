@@ -6,7 +6,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvfi_b200.so")
-SOURCES = ["tapconv.cu", "elementwise.cu", "ops.cu", "ops_extra.cu", "rife46.cu", "streamconv.cu", "film_elem.cu", "film.cu", "sepconv_elem.cu", "sepconv.cu", "gmops.cu", "flavr_elem.cu", "flavr.cu"]
+SOURCES = ["tapconv.cu", "elementwise.cu", "ops.cu", "ops_extra.cu", "rife46.cu", "streamconv.cu", "film_elem.cu", "film.cu", "sepconv_elem.cu", "sepconv.cu", "gmops.cu", "flavr_elem.cu", "flavr.cu", "ifrnet_elem.cu", "ifrnet.cu"]
 HEADERS = ["ptx.cuh", "vfi_internal.h", "hoststage.h", os.path.join("..", "..", "include", "vfi_b200.h")]
 
 

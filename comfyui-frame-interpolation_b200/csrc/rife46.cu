@@ -161,6 +161,7 @@ struct vfi_ctx {
   vfi::FilmState* film = nullptr;  // FILM weights and workspace (film.cu)
   vfi::SepState* sep = nullptr;    // Sepconv weights and workspace (sepconv.cu)
   vfi::ModelState* flavr = nullptr;  // FLAVR weights and workspace (flavr.cu)
+  vfi::ModelState* ifrnet = nullptr;  // IFRNet weights and workspace (ifrnet.cu)
 };
 
 namespace vfi {
@@ -168,6 +169,7 @@ CtxInfo ctx_info(::vfi_ctx* c) { return CtxInfo{c->device, c->num_sms, c->s_h2d,
 FilmState*& ctx_film(::vfi_ctx* c) { return c->film; }
 SepState*& ctx_sep(::vfi_ctx* c) { return c->sep; }
 ModelState*& ctx_flavr(::vfi_ctx* c) { return c->flavr; }
+ModelState*& ctx_ifrnet(::vfi_ctx* c) { return c->ifrnet; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi
 
@@ -687,6 +689,8 @@ int vfi_destroy(vfi_ctx* c) {
   film_destroy(c->film);
   delete c->flavr;
   c->flavr = nullptr;
+  delete c->ifrnet;
+  c->ifrnet = nullptr;
   c->film = nullptr;
   sepconv_destroy(c->sep);
   c->sep = nullptr;

@@ -87,11 +87,13 @@ __device__ __forceinline__ void ring_next(uint32_t& slot, uint32_t& ph, uint32_t
 }
 
 #ifndef VFI_HOST_EMU  // (tests/host_emu runs the schedule on the CPU with the checker kernel below; no wgmma there)
-// EXT = false is the FILM kernel (bias + LeakyReLU(0.2) / identity).  EXT = true adds what the Sepconv trunk needs in
-// the epilogue: a PReLU with one learned slope (a > 0 ? a : slope * a, any sign / size of slope) and a residual tensor
+// EPI = 0 is the FILM kernel (bias + LeakyReLU(0.2) / identity).  EPI = 1 adds what the Sepconv trunk needs in the
+// epilogue: a PReLU with one learned slope (a > 0 ? a : slope * a, any sign / size of slope) and a residual tensor
 // added after it (same layout as the output; it may BE the output: every thread reads its two channels before it
-// writes them).
-template <typename T, bool EXT, int N>
+// writes them).  EPI = 2 is IFRNet's (ifrnet.cu): a residual added BEFORE a PReLU with one slope per output channel,
+// and the first n_f32 output columns stored as fp32 to a separate tensor (flow, mask and residual columns are never
+// rounded to 16 bits).
+template <typename T, int EPI, int N>
 __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_constant__ StreamConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   asm volatile("griddepcontrol.launch_dependents;");  // see tapconv.cu: programmatic dependent launch
@@ -247,14 +249,30 @@ __global__ void __launch_bounds__(kSThreads, 1) streamconv_kernel(const __grid_c
         if (gy >= p.H || gx >= p.W) continue;
         const size_t opix = (((size_t)tc.b * p.H + gy) * p.W + gx) * (size_t)p.out_pitch + (size_t)n0;
         T* orow = reinterpret_cast<T*>(p.out) + opix;
-        const T* rrow = reinterpret_cast<const T*>(p.res) + opix;  // EXT only
+        const T* rrow = reinterpret_cast<const T*>(p.res) + opix;  // EPI 1, 2 only
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
           const int n = 8 * j + c2;
           const float2 sh = *reinterpret_cast<const float2*>(p.shift + n0 + n);
           float a0 = acc[h][4 * j + 2 * e] + sh.x, a1 = acc[h][4 * j + 2 * e + 1] + sh.y;
           uint32_t o;
-          if constexpr (EXT) {
+          if constexpr (EPI == 2) {
+            if (p.res != nullptr) {
+              const float2 rf = Pack2<T>::unpack(*reinterpret_cast<const uint32_t*>(rrow + n));
+              a0 += rf.x;
+              a1 += rf.y;
+            }
+            const float2 sl = *reinterpret_cast<const float2*>(p.slopes + n0 + n);
+            a0 = a0 > 0.f ? a0 : sl.x * a0;
+            a1 = a1 > 0.f ? a1 : sl.y * a1;
+            // the fp32 columns lie in the first 8 of split 0 (launch_streamconv checks n_f32 <= 8)
+            if (j == 0 && n0 + n < p.n_f32) {
+              const size_t fpix = (((size_t)tc.b * p.H + gy) * p.W + gx) * (size_t)p.f32_pitch;
+              *reinterpret_cast<float2*>(p.out_f32 + fpix + n) = make_float2(a0, a1);
+              continue;
+            }
+            o = Pack2<T>::pack(a0, a1);
+          } else if constexpr (EPI == 1) {
             a0 = a0 > 0.f ? a0 : p.slope * a0;
             a1 = a1 > 0.f ? a1 : p.slope * a1;
             if (p.res != nullptr) {
@@ -327,7 +345,14 @@ __global__ void streamconv_ref_kernel(const __grid_constant__ StreamConvParams p
     }
     float v = acc + p.shift[n];
     const size_t oidx = (((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.out_pitch + n;
-    if (p.ext) {
+    if (p.ext == 2) {
+      if (p.res != nullptr) v += sc_ld<T>(reinterpret_cast<const T*>(p.res) + oidx);
+      v = v > 0.f ? v : p.slopes[n] * v;
+      if (n < p.n_f32) {
+        p.out_f32[(((size_t)b * p.H + gy) * p.W + gx) * (size_t)p.f32_pitch + n] = v;
+        continue;
+      }
+    } else if (p.ext) {
       v = v > 0.f ? v : p.slope * v;
       if (p.res != nullptr) v += sc_ld<T>(reinterpret_cast<const T*>(p.res) + oidx);
     } else if (p.act) {
@@ -476,7 +501,7 @@ bool pack_streamconv(const StreamConvLayer& L, int op_type, const std::function<
 
 cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void* src0, int pitch0, const void* src1,
                               int pitch1, void* out, int out_pitch, int B, int H, int W, int num_sms, bool use_ref,
-                              cudaStream_t st, const void* res) {
+                              cudaStream_t st, const void* res, float* out_f32, int f32_pitch) {
   StreamConvParams p{};
   if (!streamconv_plan(L, &p)) {
     set_error("streamconv: unsupported layer shape");
@@ -504,6 +529,15 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
     set_error("streamconv: residual slice must be 32-byte aligned");
     return cudaErrorInvalidValue;
   }
+  if (L.ext == 2 && (!L.slopes || (L.n_f32 & 1) || L.n_f32 > 8 ||
+                     (L.n_f32 && (!out_f32 || ((uintptr_t)out_f32 & 7) || (f32_pitch & 1) || f32_pitch < L.n_f32)))) {
+    set_error("streamconv: an IFRNet epilogue needs its slopes, and an 8-byte aligned fp32 slice for its fp32 columns");
+    return cudaErrorInvalidValue;
+  }
+  p.slopes = L.slopes;
+  p.n_f32 = L.ext == 2 ? L.n_f32 : 0;
+  p.out_f32 = out_f32;
+  p.f32_pitch = f32_pitch;
   p.w = L.w;
   p.shift = L.shift;
   p.B = B * L.T_out;
@@ -556,9 +590,9 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, p);
   };
-  auto pick_n = [&](auto tag, auto ext) -> cudaError_t {
+  auto pick_n = [&](auto tag, auto epi) -> cudaError_t {
     using T = decltype(tag);
-    constexpr bool X = decltype(ext)::value;
+    constexpr int X = decltype(epi)::value;
     switch (p.n_cta) {  // streamconv_plan: a multiple of 16 up to 128
       case 16: return go(streamconv_kernel<T, X, 16>);
       case 32: return go(streamconv_kernel<T, X, 32>);
@@ -571,7 +605,11 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
     }
   };
   auto pick = [&](auto tag) -> cudaError_t {
-    return L.ext ? pick_n(tag, std::true_type{}) : pick_n(tag, std::false_type{});
+    switch (L.ext) {
+      case 0: return pick_n(tag, std::integral_constant<int, 0>{});
+      case 1: return pick_n(tag, std::integral_constant<int, 1>{});
+      default: return pick_n(tag, std::integral_constant<int, 2>{});
+    }
   };
   const cudaError_t err = (op_type == OP_BF16) ? pick(__nv_bfloat16{}) : pick(__half{});
   if (err != cudaSuccess) return err;

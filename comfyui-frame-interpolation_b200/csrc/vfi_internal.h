@@ -183,7 +183,10 @@ struct StreamConvLayer {
   int n_total = 0;        // output channels (multiple of 16; padded with zero weights where the layer has fewer)
   int act = 1;            // 1: LeakyReLU(0.2), 0: none
   int ext = 0;            // 1: Sepconv epilogue instead: PReLU with one learned `slope` (1.0 = none), then + residual
+                          // 2: IFRNet epilogue: + residual, then PReLU with per-channel `slopes`; columns < n_f32 fp32
   float slope = 1.f;
+  const float* slopes = nullptr;  // ext 2: device, [n_total] PReLU slopes (1.0 = identity)
+  int n_f32 = 0;                  // ext 2: output columns [0, n_f32) go to the fp32 tensor of the launch
   int pad_before = -1;    // rows / columns of zero padding before the window; -1: (ksize - 1) / 2 ('same')
   int pad_before_x = -1;  // columns of zero padding before the window when >= 0 (rows keep pad_before)
   int kt = 1, pad_t = 0;  // temporal taps and zero planes before plane 0
@@ -198,9 +201,12 @@ struct alignas(64) StreamConvParams {
   int src_pitch[2];
   void* out;              // 16-bit NHWC, channel 0 of this layer's slice
   int out_pitch;          // elements per pixel of the output tensor
-  const void* res;        // ext: residual added after the activation (layout of `out`), or nullptr
-  float slope;            // ext: PReLU slope
+  const void* res;        // ext: residual added after (ext 2: before) the activation (layout of `out`), or nullptr
+  float slope;            // ext 1: PReLU slope
   int ext;
+  const float* slopes;    // ext 2: per-channel PReLU slopes [n_total]
+  float* out_f32;         // ext 2: fp32 NHWC tensor of the columns [0, n_f32), pixel pitch f32_pitch
+  int f32_pitch, n_f32;
   const void* w;
   const float* shift;
   size_t w_split_bytes;   // packed weight bytes of one output-channel split
@@ -222,7 +228,7 @@ struct alignas(64) StreamConvParams {
 bool streamconv_plan(const StreamConvLayer& L, StreamConvParams* p_out);
 cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void* src0, int pitch0, const void* src1,
                               int pitch1, void* out, int out_pitch, int B, int H, int W, int num_sms, bool use_ref,
-                              cudaStream_t st, const void* res = nullptr);
+                              cudaStream_t st, const void* res = nullptr, float* out_f32 = nullptr, int f32_pitch = 0);
 
 // host-only operand packer (film.cu): wfun(output column n, tap = ky * k + kx, padded input channel) -> weight
 bool pack_streamconv(const StreamConvLayer& L, int op_type, const std::function<float(int, int, int)>& wfun,
@@ -296,6 +302,25 @@ cudaError_t launch_flavr_apply(int op_type, const void* x, int phases, const flo
 cudaError_t launch_flavr_outconv(int op_type, const void* x, int S, int Hp, int Wp, int H, int W, int pt, int pl,
                                  const float* w, const float* bias, const float* sums, int T, float* out, cudaStream_t st);
 
+// ---- IFRNet kernels around the convolutions (ifrnet_elem.cu); frames and output are fp32 [3][H][W] planes ----
+int ifrnet_sum_blocks();  // partial sums of launch_ifrnet_mean (doubles)
+cudaError_t launch_ifrnet_mean(const float* f0, const float* f1, int H, int W, int Hp, int Wp, double* partial, float* mean,
+                               cudaStream_t st);
+cudaError_t launch_ifrnet_prep(const float* f0, const float* f1, int H, int W, int Hp, int Wp, int h0, int w0, float scale,
+                               const float* mean, float4* out, cudaStream_t st);
+cudaError_t launch_ifrnet_first_conv(int op, const float4* xin, int h0, int w0, int h1, int w1, int k, const float* w,
+                                     const float* bias, const float* slopes, int C, int pitch, void* out, cudaStream_t st);
+cudaError_t launch_ifrnet_s2d(int op, const void* in, int pitch, int cq, int B, int h, int w, void* out, int opitch,
+                              cudaStream_t st);
+cudaError_t launch_ifrnet_dec4_in(int op, const void* f, int fpitch, int g1, int h, int w, float embt, void* out,
+                                  cudaStream_t st);
+cudaError_t launch_ifrnet_dec_flow(const float* ph, int nf, const float* prev, int h, int w, float* acc, cudaStream_t st);
+cudaError_t launch_ifrnet_dec_in(int op, const void* ph16, int pp, const void* f, int fpitch, int fh, int fw,
+                                 const float* acc, int gh, int gw, int g1, int g2, int g3, void* out, cudaStream_t st);
+cudaError_t launch_ifrnet_final(const float* f0, const float* f1, int H, int W, int Hp, int Wp, const float* acc, int hq,
+                                int wq, int hF, int wF, float scale, float fmul, const float* mean, float* out,
+                                cudaStream_t st);
+
 cudaError_t launch_adacof(const float* in, const float* weight, const float* off_i, const float* off_j, float* out, int N,
                           int C, int Hin, int Win, int F, int dil, int Ho, int Wo, cudaStream_t st);
 cudaError_t launch_edt_pass(const float* data, float* out, int bs, int h, int w, float diam2, cudaStream_t st);
@@ -318,6 +343,7 @@ void film_destroy(FilmState* f);  // film.cu
 CtxInfo ctx_info(::vfi_ctx* c);
 FilmState*& ctx_film(::vfi_ctx* c);
 ModelState*& ctx_flavr(::vfi_ctx* c);  // a FlavrState (flavr.cu)
+ModelState*& ctx_ifrnet(::vfi_ctx* c);  // an IfrnetState (ifrnet.cu)
 SepState*& ctx_sep(::vfi_ctx* c);
 void ctx_add_launches(::vfi_ctx* c, int n);
 

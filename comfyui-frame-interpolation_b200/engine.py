@@ -493,3 +493,131 @@ class FlavrEngine:
 
     def sync(self):
         check(self._L.vfi_sync(self._ctx))
+
+
+# IRFNet_S / IRFNet_L.state_dict(): pyramid channels, ResBlock side channels, first conv kernel, decoder4..1 convblock
+# channels and ConvT outputs (IFRNet_S_arch.py / IFRNet_L_arch.py)
+IFRNET_ARCH = {
+    "S": dict(enc=(24, 36, 54, 72), side=24, k0=3, dc=(144, 162, 108, 72), dout=(58, 40, 28, 8)),
+    "L": dict(enc=(64, 96, 144, 192), side=64, k0=7, dc=(384, 432, 288, 192), dout=(148, 100, 68, 8)),
+}
+
+
+def ifrnet_state_dict_spec(variant: str):
+    """IRFNet_{S,L}.state_dict() names and shapes, in order (104 tensors)."""
+    a = IFRNET_ARCH[variant]
+    spec, cin = [], 3
+    for l, co in enumerate(a["enc"]):
+        for j in range(2):
+            k = a["k0"] if (l == 0 and j == 0) else 3
+            p = f"encoder.pyramid{l + 1}.{j}."
+            spec += [(p + "0.weight", (co, cin if j == 0 else co, k, k)), (p + "0.bias", (co,)), (p + "1.weight", (co,))]
+        cin = co
+    for k in range(4):
+        p = f"decoder{4 - k}.convblock."
+        C, s = a["dc"][k], a["side"]
+        ci = 2 * a["enc"][3] + 1 if k == 0 else a["dout"][k - 1] + 2 * a["enc"][3 - k]
+        spec += [(p + "0.0.weight", (C, ci, 3, 3)), (p + "0.0.bias", (C,)), (p + "0.1.weight", (C,))]
+        for j in range(1, 5):
+            n = s if j in (2, 4) else C
+            spec += [(p + f"1.conv{j}.0.weight", (n, n, 3, 3)), (p + f"1.conv{j}.0.bias", (n,)), (p + f"1.conv{j}.1.weight", (n,))]
+        spec += [(p + "1.conv5.weight", (C, C, 3, 3)), (p + "1.conv5.bias", (C,)), (p + "1.prelu.weight", (C,))]
+        spec += [(p + "2.weight", (C, a["dout"][k], 4, 4)), (p + "2.bias", (a["dout"][k],))]
+    return spec
+
+
+def ifrnet_geometry(h: int, w: int, t: float):
+    """The sizes vfi_ifrnet_forward uses for an h x w frame at resize factor t (the reference's arithmetic), as a dict;
+    raises VfiError for a t the reference cannot run (an empty encoder input, an output smaller than the frame)."""
+    v = np.zeros(22, np.int32)
+    check(lib().vfi_ifrnet_geometry(int(h), int(w), float(t), v.ctypes.data, 22))
+    keys = ("hp", "wp", "h0", "w0", "h1", "w1", "h2", "w2", "h3", "w3", "h4", "w4", "dh3", "dw3", "dh2", "dw2", "dh1", "dw1",
+            "hq", "wq", "hf", "wf")
+    return dict(zip(keys, [int(x) for x in v]))
+
+
+class IfrnetEngine:
+    """IFRNet-S / IFRNet-L (IFRNet_{S,L}_{Vimeo90K,GoPro}.pth) on one H100: `state_dict` = IRFNet_S's or IRFNet_L's; the
+    variant is read from the shapes and every shape is checked.  fp16 operands with fp32 accumulation ("float32", as the
+    node runs it); flows, mask, warps and the blend are fp32."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, dtype: str = "float32"):
+        if not torch.cuda.is_available():
+            raise VfiError("no CUDA device: this path has no CPU fallback")
+        if dtype not in OPERAND:
+            raise ValueError(f"dtype must be one of {list(OPERAND)}")
+        first = state_dict.get("encoder.pyramid1.0.0.weight")
+        if first is None:
+            raise KeyError("state_dict is not an IFRNet checkpoint; missing encoder.pyramid1.0.0.weight")
+        variant = "L" if tuple(first.shape[-2:]) == (7, 7) else "S"
+        spec = ifrnet_state_dict_spec(variant)
+        for name, shape in spec:
+            if name not in state_dict:
+                raise KeyError(f"state_dict is not an IFRNet-{variant} checkpoint; missing {name}")
+            if tuple(state_dict[name].shape) != shape:
+                raise ValueError(f"IFRNet-{variant}: {name} has shape {tuple(state_dict[name].shape)}, expected {shape}")
+        self._L = lib()
+        self.device = int(device)
+        self._ctx = C.c_void_p()
+        check(self._L.vfi_create(self.device, C.byref(self._ctx)))
+        hold = [state_dict[n].detach().to("cpu", torch.float32).contiguous() for n, _ in spec]
+        ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+        numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+        check(self._L.vfi_ifrnet_load(self._ctx, ptrs, numel, len(hold), OPERAND[dtype]))
+        v = C.c_int()
+        check(self._L.vfi_ifrnet_info(self._ctx, C.byref(v)))
+        self.variant = "L" if v.value else "S"
+        self.dtype = dtype
+
+    def close(self):
+        if getattr(self, "_ctx", None) is not None and self._ctx.value:
+            self._L.vfi_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def forward(self, img0: torch.Tensor, img1: torch.Tensor, t: float, embt: float,
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """img0, img1: CUDA float32 [1, 3, H, W] -> [1, 3, H, W] = model(img0, img1, scale_factor=t, timestep=embt)."""
+        for x in (img0, img1):
+            assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4 and x.shape[:2] == (1, 3)
+        assert img0.shape == img1.shape
+        _, _, h, w = img0.shape
+        if out is None:
+            out = torch.empty((1, 3, h, w), dtype=torch.float32, device=img0.device)
+        assert out.is_cuda and out.is_contiguous() and out.dtype == torch.float32 and out.shape == img0.shape
+        st = torch.cuda.current_stream(img0.device).cuda_stream
+        check(self._L.vfi_ifrnet_forward(self._ctx, img0.data_ptr(), img1.data_ptr(), h, w, float(t), float(embt),
+                                         out.data_ptr(), st))
+        return out
+
+    # ------------------------------------------------------------------ hooks
+    def set_ref(self, use_ref: bool):
+        check(self._L.vfi_ifrnet_debug_set_ref(self._ctx, 1 if use_ref else 0))
+
+    def debug_conv(self, layer, src0, pitch0, src1, pitch1, out, out_pitch, n_images, H, W, impl=0, res=None,
+                   out_f32=None, f32_pitch=0):
+        """One conv layer on raw tensors (pointers with element offsets already applied by the caller's views)."""
+        st = torch.cuda.current_stream(src0.device).cuda_stream
+        check(self._L.vfi_ifrnet_debug_conv(
+            self._ctx, layer, src0.data_ptr(), int(pitch0), None if src1 is None else src1.data_ptr(), int(pitch1),
+            out.data_ptr(), int(out_pitch), None if res is None else res.data_ptr(),
+            None if out_f32 is None else out_f32.data_ptr(), int(f32_pitch), n_images, H, W, impl, st))
+        return out
+
+    def layer_plan(self, layer):
+        v = np.zeros(12, np.int32)
+        check(self._L.vfi_ifrnet_layer_plan(self._ctx, layer, v.ctypes.data, 12))
+        keys = ("c0", "c1", "n_total", "ksize", "pad_y", "pad_x", "n_cta", "nsplit", "a_slots", "b_slots", "smem_bytes",
+                "n_f32")
+        return dict(zip(keys, [int(x) for x in v]))
+
+    def launch_count(self) -> int:
+        return int(self._L.vfi_launch_count(self._ctx))
+
+    def sync(self):
+        check(self._L.vfi_sync(self._ctx))

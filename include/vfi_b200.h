@@ -204,6 +204,33 @@ int vfi_flavr_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0, 
 int vfi_flavr_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
 int vfi_flavr_info(vfi_ctx* ctx, int* n_outputs, int* enc_bias);
 
+/* IFRNet (`IFRNet VFI` node: IRFNet_S / IRFNet_L) ---------------------------------------------------------- */
+#define VFI_IFRNET_NUM_TENSORS 104
+/* Replaces: IRFNet_S() / IRFNet_L() + load_state_dict (ifrnet/__init__.py:44-45).  HOST float32 arrays in
+ * state_dict() order (engine.py ifrnet_state_dict_spec); the variant is read from the first tensor's size, and every
+ * tensor's size is checked against it. */
+int vfi_ifrnet_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type);
+/* Replaces: `model(img0, img1, scale_factor=t, timestep=embt)` for one pair (IRFNet_S.forward).  DEVICE pointers: img0,
+ * img1 and out are float32 [3][H][W] planes (NCHW, batch 1); out is clamped to [0, 1].  t is the resize factor of the
+ * encoder input, embt the value of decoder 4's time plane.  Sizes follow the reference's arithmetic; a t that gives an
+ * empty encoder input or an output smaller than the frame is refused before any launch.  Asynchronous on `stream`. */
+int vfi_ifrnet_forward(vfi_ctx* ctx, const float* img0, const float* img1, int H, int W, double t, double embt, float* out,
+                       void* stream);
+/* The sizes vfi_ifrnet_forward would use (no context): {Hp, Wp, encoder input h, w, levels 1..4 h, w, decoder 3..1 grids
+ * h, w, decoder 1 output h, w, final resize h, w} (22 values), or the error it would return. */
+int vfi_ifrnet_geometry(int H, int W, double t, int32_t* info, int cap);
+/* Test hooks: every conv through the CUDA-core checker (1) / the wgmma kernel (0); run one conv layer (id: encoder
+ * 0..6 = pyramid1.1, pyramid2.0 (stride 2, space-to-depth input), pyramid2.1, ..; decoder k = 0 (decoder4) .. 3:
+ * 10 + 10 k + {0 convblock.0, 1..5 ResBlock conv1..conv5, 6..9 ConvT phase py * 2 + px}); its plan
+ * {c0, c1, n_total, ksize, pad_y, pad_x, n_cta, nsplit, a_slots, b_slots, smem_bytes, n_f32}; the loaded variant
+ * (0: IFRNet-S, 1: IFRNet-L). */
+int vfi_ifrnet_debug_set_ref(vfi_ctx* ctx, int use_ref);
+int vfi_ifrnet_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0, const void* src1, int pitch1, void* out,
+                          int out_pitch, const void* res, float* out_f32, int f32_pitch, int n_images, int H, int W,
+                          int impl, void* stream);
+int vfi_ifrnet_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
+int vfi_ifrnet_info(vfi_ctx* ctx, int* variant);
+
 /* Test / profiling hooks (used by tests/ and bench.py only) --------------------------------------------- */
 /* Run ONE convolution layer of block `block` (0..3; arch 4.26: 0..4): layer 0 = conv0.0, 1 = conv0.1, 2..9 = ResConv
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
