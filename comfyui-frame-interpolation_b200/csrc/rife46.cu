@@ -78,9 +78,10 @@ std::vector<uint16_t> pack_weights(const TapConvLayer& L, int op_type, F wfun) {
   return v;
 }
 
-// choose the output-channel split: smallest split reaching `want_stages`, else the one with most stages
-void choose_split(TapConvLayer& L, const std::vector<int>& splits, int want_stages) {
-  int best_split = -1, best_stages = 0;
+// choose the output-channel split: smallest split reaching `want_stages`, else the one with most stages; returns its
+// stages (0: no split fits in shared memory)
+int choose_split(TapConvLayer& L, const std::vector<int>& splits, int want_stages) {
+  int best_split = 1, best_stages = 0;
   for (int sp : splits) {
     if (L.n_total % sp) continue;
     const int nc = L.n_total / sp;
@@ -101,6 +102,49 @@ void choose_split(TapConvLayer& L, const std::vector<int>& splits, int want_stag
   }
   L.nsplit = best_split;
   L.n_cta = L.n_total / best_split;
+  return best_stages;
+}
+
+// Tap-conv layer roles.  An IFBlock's layers are vfi_ctx::layers[block][role], numbered as in the C ABI
+// (vfi_rife46_debug_layer, vfi_rife46_layer_plan); the Head's layers of arch 4.17 / 4.26 are vfi_ctx::head[].
+enum LayerRole : int {
+  LAYER_CONV00 = 0,      // conv0.0: stride 2 over the space-to-depth block input, space-to-depth output
+  LAYER_CONV01 = 1,      // conv0.1: stride 2 over conv0.0's output
+  LAYER_RESCONV = 2,     // the eight ResConvs: LAYER_RESCONV + j, j < 8
+  LAYER_LASTCONV = 10,   // ConvTranspose2d + PixelShuffle: flow + mask
+  LAYER_LASTFEAT = 11,   // arch 4.26: the 8 feature channels of lastconv, for the next block (not in the last block)
+  LAYER_HEAD_CONV = 12,  // Head cnn1 / cnn2: 3x3 + LeakyReLU
+  LAYER_HEAD_DECONV,     // Head cnn3: ConvTranspose2d(4, 2, 1), output in space-to-depth form
+};
+constexpr int kBlockLayers = LAYER_LASTFEAT + 1;
+
+// How a layer of a role with `ch` input channels runs.  A streamed layer (wstream, tapconv.cu) lists its one fixed
+// output-channel split; a resident layer takes the first of `splits` whose plan reaches `want_stages` window stages,
+// else the one with the most.
+struct LayerSpec {
+  int epi_mode, out_s2d, wstream;
+  std::vector<int> splits;
+  int want_stages;
+};
+
+LayerSpec layer_spec(int role, int ch) {
+  const std::vector<int> div12 = {1, 2, 3, 4, 6, 8, 12};  // the splits of the resident conv0 / ResConv layers
+  switch (role) {  // {epi_mode, out_s2d, wstream, splits, want_stages}
+    case LAYER_CONV00: return {EPI_BIAS_LRELU, 1, 0, div12, 2};
+    case LAYER_CONV01: return {EPI_BIAS_LRELU, 0, 0, div12, 2};
+    case LAYER_RESCONV:  // streamed: all channels per CTA up to the wgmma's N = 128, else two halves
+      return ch >= 96 ? LayerSpec{EPI_RESCONV, 0, 1, {ch > 128 ? 2 : 1}, 1} : LayerSpec{EPI_RESCONV, 0, 0, div12, 3};
+    case LAYER_LASTCONV: return ch == 128 ? LayerSpec{EPI_LASTCONV, 0, 1, {1}, 1} : LayerSpec{EPI_LASTCONV, 0, 0, {1, 5}, 2};
+    case LAYER_LASTFEAT: return ch >= 128 ? LayerSpec{EPI_BIAS, 2, 1, {1}, 1} : LayerSpec{EPI_BIAS, 2, 0, {2, 4, 8}, 2};
+    case LAYER_HEAD_CONV: return {EPI_BIAS_LRELU, 0, 0, {1}, 2};
+    default: return {EPI_BIAS, 0, 0, {1}, 2};  // LAYER_HEAD_DECONV
+  }
+}
+
+// whether the loaded arch has this block layer: LAYER_LASTFEAT only in arch 4.26, in every block but the last
+bool block_has_layer(int arch, int block, int layer) {
+  const int nb = num_blocks(arch);
+  return block < nb && layer < kBlockLayers && (layer != LAYER_LASTFEAT || (arch == 426 && block + 1 < nb));
 }
 
 struct DevBuf {
@@ -134,8 +178,7 @@ struct vfi_ctx {
   int op_type = OP_F16;
   bool loaded = false;
   int64_t launches = 0;
-  TapConvLayer layers[kMaxBlocks][12];  // [block][0=conv0.0, 1=conv0.1, 2..9=ResConv, 10=lastconv (flow + mask),
-                                        //          11 = arch 4.26: the 8 feature channels of lastconv]
+  TapConvLayer layers[kMaxBlocks][kBlockLayers];  // [block][LayerRole]
   std::vector<void*> weight_allocs;
   // workspace
   DevBuf imgs, imgs_h, flow, mask, x, c00, featA, featB, tF[kMaxBlocks], tM[kMaxBlocks], raw, outdev;
@@ -205,237 +248,87 @@ int upload(vfi_ctx* c, const std::vector<T>& h, void** dptr) {
   return VFI_OK;
 }
 
-// stride-2 3x3 conv on a space-to-depth input: kernel row ky reads s2d row offset dy and sub-row a
-void s2_map(int k, int* d, int* a) {
-  if (k == 0) { *d = -1; *a = 1; } else { *d = 0; *a = k - 1; }
+// A layer's weights as a function of (kernel tap ky*3 + kx, input channel, output column), and its shift per column.
+struct WeightMap {
+  std::function<float(int tap, int ci, int n)> w;
+  std::function<float(int n)> shift;
+};
+
+// Conv2d(creal -> nreal, 3x3) [nreal][creal][3][3] + bias; input channels and columns past the real ones are zero
+// padding.  `beta` (ResConv): (conv(x) + b) * beta + x == conv_{w*beta}(x) + b*beta + x - beta is folded into the packed
+// weights (one 16-bit rounding of w*beta instead of w) so the epilogue is a pure add.
+WeightMap conv2d(const float* w, const float* bias, int creal, int nreal, const float* beta = nullptr) {
+  return {[=](int tap, int ci, int n) {
+            return ci < creal && n < nreal ? w[((size_t)n * creal + ci) * 9 + tap] * (beta ? beta[n] : 1.f) : 0.f;
+          },
+          [=](int n) { return n < nreal ? bias[n] * (beta ? beta[n] : 1.f) : 0.f; }};
 }
 
-int build_conv_s2(vfi_ctx* c, TapConvLayer& L, int Cs, int creal, int cout, int out_s2d, const float* w,
-                  const float* bias) {
+// Column n of a ConvTranspose2d(4, 2, 1) run as a 3x3 tap conv: channel oc at sub-pixel (a, b) of the 2x2 block an input
+// cell (y, x) covers, output position (2y + a, 2x + b).
+struct ConvTCol { int oc, a, b; };
+
+// ConvTranspose2d(creal -> cout, 4, 2, 1) [creal][cout][4][4] + bias as ONE 3x3 conv on the input grid: tap (dy, dx)
+// of column n uses transposed-kernel element ky = a+1-2dy, kx = b+1-2dx (no weight outside the 4x4 kernel).
+WeightMap conv_transpose(const float* wt, const float* bias, int creal, int cout, std::function<ConvTCol(int)> col) {
+  return {[=](int tap, int ci, int n) {
+            const ConvTCol k = col(n);
+            const int ky = k.a + 1 - 2 * (tap / 3 - 1), kx = k.b + 1 - 2 * (tap % 3 - 1);
+            if (ci >= creal || ky < 0 || ky > 3 || kx < 0 || kx > 3) return 0.f;
+            return wt[(((size_t)ci * cout + k.oc) * 4 + ky) * 4 + kx];
+          },
+          [=](int n) { return bias[col(n).oc]; }};
+}
+
+// ConvTranspose2d + PixelShuffle(2): channel c at sub-pixel (py, px) of an input cell's 4x4 patch
+ConvTCol shuffled(int c, int py, int px) { return {4 * c + 2 * (py & 1) + (px & 1), py >> 1, px >> 1}; }
+
+// One tap-conv layer of `role` over `ch` input channels (conv0.0 / conv0.1: per space-to-depth sub-pixel) with n_total
+// output columns: its taps, the plan of layer_spec, and its packed weights and shift uploaded.
+int build_layer(vfi_ctx* c, TapConvLayer& L, int role, int ch, int n_total, const WeightMap& wm) {
+  const LayerSpec s = layer_spec(role, ch);
+  const bool s2 = role == LAYER_CONV00 || role == LAYER_CONV01;
+  // a streamed layer over whole 64-channel k-blocks takes k-block-major (kb, tap) entries, else one entry per tap over all
+  // channels; the packed weights follow the same K order
+  const int nkb = s.wstream && ch % 64 == 0 ? ch / 64 : 1;
   L = TapConvLayer{};
-  L.cin = 4 * Cs;
-  L.n_total = cout;
-  L.ntaps = 9;
-  L.ktotal16 = 9 * (Cs / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 1; L.halo_w = kTileW + 1;
-  L.epi_mode = EPI_BIAS_LRELU;
-  L.out_s2d = out_s2d;
-  for (int ky = 0; ky < 3; ++ky)
-    for (int kx = 0; kx < 3; ++kx) {
-      int dy, a, dx, b;
-      s2_map(ky, &dy, &a);
-      s2_map(kx, &dx, &b);
-      TapEntry& t = L.taps[ky * 3 + kx];
-      t.dy = (int16_t)dy; t.dx = (int16_t)dx;
-      t.chunk0 = (int16_t)(((a * 2 + b) * Cs) / 8);
-      t.nk16 = (int16_t)(Cs / 16);
-    }
-  choose_split(L, {1, 2, 3, 4, 6, 8, 12}, 2);
-  auto wf = [&](int e, int ci, int n) -> float {
-    if (ci >= creal) return 0.f;
-    const int ky = e / 3, kx = e % 3;
-    return w[(((size_t)n * creal + ci) * 3 + ky) * 3 + kx];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(bias, bias + cout);
-  int r;
-  if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
-}
-
-// 3x3 taps over all `ch` input channels.  kb_major: k-block-major (kb, tap) entries of 64 channels each (ch % 64 == 0),
-// else one entry per tap over all channels; the packed weights follow the same order.
-void set_taps_3x3(TapConvLayer& L, int ch, bool kb_major) {
-  const int nkb = kb_major ? ch / 64 : 1;
+  L.cin = s2 ? 4 * ch : ch;
+  L.n_total = n_total;
   L.ntaps = 9 * nkb;
+  L.ktotal16 = 9 * (ch / 16);
+  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + (s2 ? 1 : 2); L.halo_w = kTileW + (s2 ? 1 : 2);
+  L.epi_mode = s.epi_mode;
+  L.out_s2d = s.out_s2d;
+  L.wstream = s.wstream;
   for (int kb = 0; kb < nkb; ++kb)
     for (int e = 0; e < 9; ++e) {
       TapEntry& t = L.taps[kb * 9 + e];
-      t.dy = (int16_t)(e / 3 - 1);
-      t.dx = (int16_t)(e % 3 - 1);
-      t.chunk0 = (int16_t)(kb * 8);
-      t.nk16 = (int16_t)(kb_major ? 4 : ch / 16);
+      const int ky = e / 3, kx = e % 3;
+      t.nk16 = (int16_t)(ch / 16 / nkb);
+      if (s2) {  // input row 2y + ky - 1 = 2(y + dy) + a: space-to-depth row offset dy, sub-row a (columns alike)
+        const int a = ky == 0 ? 1 : ky - 1, b = kx == 0 ? 1 : kx - 1;
+        t.dy = (int16_t)(ky == 0 ? -1 : 0); t.dx = (int16_t)(kx == 0 ? -1 : 0);
+        t.chunk0 = (int16_t)((a * 2 + b) * ch / 8);
+      } else {
+        t.dy = (int16_t)(ky - 1); t.dx = (int16_t)(kx - 1);
+        t.chunk0 = (int16_t)(kb * 8);
+      }
     }
-}
-
-int build_resconv(vfi_ctx* c, TapConvLayer& L, int ch, const float* beta, const float* w, const float* bias) {
-  L = TapConvLayer{};
-  L.cin = ch;
-  L.n_total = ch;
-  L.ntaps = 9;
-  L.ktotal16 = 9 * (ch / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
-  L.epi_mode = EPI_RESCONV;
-  int real_taps = 9;
-  if (ch >= 96) {
-    // streamed weights (tapconv.cu): all channels per CTA up to the wgmma's N = 128, else two halves of 96.  The taps
-    // keep the K order of the resident-weight plans: k-block-major at c = 128 / 192, tap-major at c = 96.
-    set_taps_3x3(L, ch, ch % 64 == 0);
-    real_taps = L.ntaps;
-    L.wstream = 1;
-    L.nsplit = ch > 128 ? 2 : 1;
-    L.n_cta = ch / L.nsplit;
-    if (L.ktotal16 & 3) {  // c = 96: 54 K=16 steps; two more with zero weights fill the last four-step weight slot
-      TapEntry& t = L.taps[L.ntaps++];
-      t.dy = 0; t.dx = 0; t.chunk0 = 0;
-      t.nk16 = (int16_t)(4 - (L.ktotal16 & 3));
-      L.ktotal16 += t.nk16;
-    }
-  } else {
-    set_taps_3x3(L, ch, false);
-    choose_split(L, {1, 2, 3, 4, 6, 8, 12}, 3);
+  const int real_taps = L.ntaps;
+  if (s.wstream && (L.ktotal16 & 3)) {  // zero-weight K=16 steps complete the last four-step weight slot (c = 96: 54 + 2)
+    TapEntry& t = L.taps[L.ntaps++];  // dy = dx = chunk0 = 0
+    t.nk16 = (int16_t)(4 - (L.ktotal16 & 3));
+    L.ktotal16 += t.nk16;
   }
-  // (conv(x) + b) * beta + x  ==  conv_{w*beta}(x) + b*beta + x : beta is folded into the packed weights (one 16-bit
-  // rounding of w*beta instead of w) so the epilogue is a pure add
-  auto wf = [&](int e, int ci, int n) -> float {  // e = kb * 9 + tap (kb = 0 if tap-major), ci relative to the k-block
-    if (e >= real_taps) return 0.f;
-    const int tap = e % 9, cin = (e / 9) * 64 + ci;
-    return w[(((size_t)n * ch + cin) * 3 + tap / 3) * 3 + tap % 3] * beta[n];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(ch);
-  for (int i = 0; i < ch; ++i) sh[i] = bias[i] * beta[i];
+  if (choose_split(L, s.splits, s.want_stages) < 1) return fail(VFI_E_STATE, "a layer has no shared-memory plan");
+  std::vector<uint16_t> pk = pack_weights(L, c->op_type, [&](int e, int ci, int n) {  // ci relative to the k-block
+    return e < real_taps ? wm.w(e % 9, (e / 9) * 64 + ci, n) : 0.f;
+  });
+  std::vector<float> sh(n_total);
+  for (int n = 0; n < n_total; ++n) sh[n] = wm.shift(n);
   int r;
   if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
-}
-
-// ConvTranspose2d(c, 24, 4, 2, 1) + PixelShuffle(2) as ONE 3x3 conv producing, per feature cell, the 4x4 sub-pixel
-// patch of the 5 used channels: n = c5*16 + py*4 + px, (py,px) = (2a+i, 2b+j), convT channel oc = 4*c5 + 2i + j at
-// convT position (2y+a, 2x+b); tap (dy,dx) uses transposed-kernel element ky = a+1-2dy, kx = b+1-2dx.
-int build_lastconv(vfi_ctx* c, TapConvLayer& L, int ch, int cout, const float* wt, const float* bias) {
-  L = TapConvLayer{};
-  L.cin = ch;
-  L.n_total = 80;
-  L.ntaps = 9;
-  L.ktotal16 = 9 * (ch / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
-  L.epi_mode = EPI_LASTCONV;
-  if (ch == 128) {  // streamed weights (tapconv.cu), all 80 columns in one CTA
-    set_taps_3x3(L, ch, true);
-    L.wstream = 1;
-    L.nsplit = 1;
-    L.n_cta = 80;
-  } else {
-    set_taps_3x3(L, ch, false);
-    choose_split(L, {1, 5}, 2);
-  }
-  auto oc_of = [](int n) {
-    const int c5 = n >> 4, pos = n & 15, py = pos >> 2, px = pos & 3;
-    return 4 * c5 + 2 * (py & 1) + (px & 1);
-  };
-  auto wf = [&](int e, int cr, int n) -> float {  // e = kb * 9 + tap, cr relative to the k-block
-    const int tap = e % 9, ci = (e / 9) * 64 + cr;
-    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-    const int pos = n & 15, py = pos >> 2, px = pos & 3;
-    const int ky = (py >> 1) + 1 - 2 * dy, kx = (px >> 1) + 1 - 2 * dx;
-    if (ky < 0 || ky > 3 || kx < 0 || kx > 3) return 0.f;
-    return wt[(((size_t)ci * cout + oc_of(n)) * 4 + ky) * 4 + kx];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(80);
-  for (int n = 0; n < 80; ++n) sh[n] = bias[oc_of(n)];
-  int r;
-  if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
-}
-
-// arch 4.26: channels 5..12 of ConvTranspose2d(c, 52, 4, 2, 1) + PixelShuffle(2) (rife_arch.py:230-233, :272) - the 8
-// feature channels handed to the next block - as a second 3x3 tap conv over the same input: column
-// n = (py*4 + px)*8 + f holds feature f at sub-pixel (py, px) of the cell's 4x4 patch, so 16 consecutive columns are
-// two x-adjacent sub-pixels x 8 channels = 32 contiguous bytes of the [B, 4H, 4W, 8] output (out_s2d = 2).
-int build_lastfeat(vfi_ctx* c, TapConvLayer& L, int ch, int cout, const float* wt, const float* bias) {
-  L = TapConvLayer{};
-  L.cin = ch;
-  L.n_total = 128;
-  L.ntaps = 9;
-  L.ktotal16 = 9 * (ch / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
-  L.epi_mode = EPI_BIAS;
-  L.out_s2d = 2;
-  if (ch >= 128) {  // streamed weights (tapconv.cu), all 128 columns in one CTA
-    set_taps_3x3(L, ch, true);
-    L.wstream = 1;
-    L.nsplit = 1;
-    L.n_cta = 128;
-  } else {
-    set_taps_3x3(L, ch, false);
-    choose_split(L, {2, 4, 8}, 2);
-  }
-  auto oc_of = [](int n) {
-    const int f = n & 7, pos = n >> 3, py = pos >> 2, px = pos & 3;
-    return 4 * (5 + f) + 2 * (py & 1) + (px & 1);
-  };
-  auto wf = [&](int e, int cr, int n) -> float {  // e = kb * 9 + tap, cr relative to the k-block
-    const int tap = e % 9, ci = (e / 9) * 64 + cr;
-    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-    const int pos = n >> 3, py = pos >> 2, px = pos & 3;
-    const int ky = (py >> 1) + 1 - 2 * dy, kx = (px >> 1) + 1 - 2 * dx;
-    if (ky < 0 || ky > 3 || kx < 0 || kx > 3) return 0.f;
-    return wt[(((size_t)ci * cout + oc_of(n)) * 4 + ky) * 4 + kx];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(128);
-  for (int n = 0; n < 128; ++n) sh[n] = bias[oc_of(n)];
-  int r;
-  if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
-}
-
-// Head_417.cnn1 / cnn2: plain 3x3 conv + LeakyReLU on a 32-channel half-resolution tensor (one 32-channel k-block).
-// `creal` < ch: arch 4.26's 16-channel Head layers run zero-padded to 32 channels (the kernel's smallest k-block).
-int build_conv3x3_lrelu(vfi_ctx* c, TapConvLayer& L, int ch, int creal, const float* w, const float* bias) {
-  L = TapConvLayer{};
-  L.cin = ch;
-  L.n_total = ch;
-  L.ktotal16 = 9 * (ch / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
-  L.epi_mode = EPI_BIAS_LRELU;
-  set_taps_3x3(L, ch, false);
-  choose_split(L, {1}, 2);
-  auto wf = [&](int e, int ci, int n) -> float {
-    if (ci >= creal || n >= creal) return 0.f;
-    return w[(((size_t)n * creal + ci) * 3 + e / 3) * 3 + e % 3];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(ch, 0.f);
-  for (int i = 0; i < creal; ++i) sh[i] = bias[i];
-  int r;
-  if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
-}
-
-// Head_417.cnn3 = ConvTranspose2d(ch, cout, 4, 2, 1), no activation, as ONE 3x3 conv producing the 2x2 sub-pixels of
-// every input cell: n = (a*2 + b)*cout + oc at output position (2y+a, 2x+b); tap (dy,dx) uses transposed-kernel element
-// ky = a+1-2dy, kx = b+1-2dx.  The NHWC output [Hh][Wh][4*cout] IS the space-to-depth form of the feature map.
-int build_deconv_s2d(vfi_ctx* c, TapConvLayer& L, int ch, int creal, int cout, const float* wt, const float* bias) {
-  L = TapConvLayer{};
-  L.cin = ch;
-  L.n_total = 4 * cout;
-  L.ktotal16 = 9 * (ch / 16);
-  L.halo_y0 = -1; L.halo_x0 = -1; L.halo_h = kTileH + 2; L.halo_w = kTileW + 2;
-  L.epi_mode = EPI_BIAS;
-  set_taps_3x3(L, ch, false);
-  choose_split(L, {1}, 2);
-  auto wf = [&](int e, int ci, int n) -> float {
-    const int dy = e / 3 - 1, dx = e % 3 - 1;
-    const int sub = n / cout, oc = n % cout, a = sub >> 1, b = sub & 1;
-    const int ky = a + 1 - 2 * dy, kx = b + 1 - 2 * dx;
-    if (ky < 0 || ky > 3 || kx < 0 || kx > 3 || ci >= creal) return 0.f;
-    return wt[(((size_t)ci * cout + oc) * 4 + ky) * 4 + kx];
-  };
-  std::vector<uint16_t> pk = pack_weights(L, c->op_type, wf);
-  std::vector<float> sh(4 * cout);
-  for (int n = 0; n < 4 * cout; ++n) sh[n] = bias[n % cout];
-  int r;
-  if ((r = upload(c, pk, &L.w))) return r;
-  if ((r = upload(c, sh, (void**)&L.shift))) return r;
-  return VFI_OK;
+  return upload(c, sh, (void**)&L.shift);
 }
 
 struct Geometry {
@@ -481,7 +374,7 @@ int ensure_workspace(vfi_ctx* c, const Geometry& g, int B, int n_frames_window) 
     feat = std::max(feat, (size_t)B * (Hs / 4) * (Ws / 4) * kBlockC[i] * 2);
     CK(c->tF[i].ensure((size_t)B * Hs * Ws * sizeof(float4)));  // block output T_i (flow increments at 1/s_i)
     CK(c->tM[i].ensure((size_t)B * Hs * Ws * sizeof(float)));
-    if (c->arch == 426 && i + 1 < g.nb) CK(c->tE[i].ensure((size_t)B * Hs * Ws * 16));
+    if (block_has_layer(c->arch, i, LAYER_LASTFEAT)) CK(c->tE[i].ensure((size_t)B * Hs * Ws * 16));
   }
   const size_t px = (size_t)g.Hp * g.Wp;
   CK(c->imgs.ensure((size_t)n_frames_window * px * sizeof(float4)));
@@ -602,27 +495,27 @@ int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, 
     }
     span_end();
     span_begin(10 * i + 1);
-    LAUNCH(launch_tapconv(c->layers[i][0], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, B, Hs / 2, Ws / 2,
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV00], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, B, Hs / 2, Ws / 2,
                           c->num_sms, TAPCONV_PLANNED, st));
     span_end();
     span_begin(10 * i + 2);
-    LAUNCH(launch_tapconv(c->layers[i][1], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, B, Hs / 4, Ws / 4,
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV01], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, B, Hs / 4, Ws / 4,
                           c->num_sms, TAPCONV_PLANNED, st));
     span_end();
     void* a = c->featA.p;
     void* b = c->featB.p;
     span_begin(10 * i + 3);
     for (int j = 0; j < 8; ++j) {
-      LAUNCH(launch_tapconv(c->layers[i][2 + j], c->op_type, a, b, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
+      LAUNCH(launch_tapconv(c->layers[i][LAYER_RESCONV + j], c->op_type, a, b, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
                             TAPCONV_PLANNED, st));
       std::swap(a, b);
     }
     span_end();
     span_begin(10 * i + 4);
-    LAUNCH(launch_tapconv(c->layers[i][10], c->op_type, a, nullptr, fs.f[i], fs.m[i], B, Hs / 4, Ws / 4, c->num_sms,
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTCONV], c->op_type, a, nullptr, fs.f[i], fs.m[i], B, Hs / 4, Ws / 4, c->num_sms,
                           TAPCONV_PLANNED, st));
-    if (c->arch == 426 && i + 1 < nb)  // the 8 feature channels of lastconv, for the next block's input
-      LAUNCH(launch_tapconv(c->layers[i][11], c->op_type, a, c->tE[i].p, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
+    if (block_has_layer(c->arch, i, LAYER_LASTFEAT))  // the 8 feature channels of lastconv, for the next block's input
+      LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTFEAT], c->op_type, a, c->tE[i].p, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
                             TAPCONV_PLANNED, st));
     if (g.k[i] > 1) {  // the up-scaled block's output goes straight back onto the dense planes
       LAUNCH(launch_fold_down(fs.f[i], fs.m[i], g.k[i], F, M, B, g.Hp, g.Wp, fs.mask_replace, st));
@@ -800,22 +693,50 @@ int vfi_rife_load(vfi_ctx* c, int arch, const float* const* T, const int64_t* nu
     if (!expect(k, (int64_t)(ch / 2) * cin * 9) || !expect(k + 1, ch / 2) || !expect(k + 2, (int64_t)ch * (ch / 2) * 9) ||
         !expect(k + 3, ch))
       return fail(VFI_E_INVALID, "conv0 tensor sizes do not match RIFE 4.6");
+    TapConvLayer* Lb = c->layers[b];
     int r;
-    if ((r = build_conv_s2(c, c->layers[b][0], arch != 46 ? 32 : 16, cin, ch / 2, 1, T[k], T[k + 1]))) return r;
-    if ((r = build_conv_s2(c, c->layers[b][1], ch / 2, ch / 2, ch, 0, T[k + 2], T[k + 3]))) return r;
+    if ((r = build_layer(c, Lb[LAYER_CONV00], LAYER_CONV00, arch != 46 ? 32 : 16, ch / 2,
+                         conv2d(T[k], T[k + 1], cin, ch / 2))))
+      return r;
+    if ((r = build_layer(c, Lb[LAYER_CONV01], LAYER_CONV01, ch / 2, ch, conv2d(T[k + 2], T[k + 3], ch / 2, ch))))
+      return r;
     k += 4;
     for (int j = 0; j < 8; ++j) {
       if (!expect(k, ch) || !expect(k + 1, (int64_t)ch * ch * 9) || !expect(k + 2, ch))
         return fail(VFI_E_INVALID, "convblock tensor sizes do not match RIFE 4.6");
-      if ((r = build_resconv(c, c->layers[b][2 + j], ch, T[k], T[k + 1], T[k + 2]))) return r;
+      if ((r = build_layer(c, Lb[LAYER_RESCONV + j], LAYER_RESCONV, ch, ch, conv2d(T[k + 1], T[k + 2], ch, ch, T[k]))))
+        return r;
       k += 3;
     }
     if (!expect(k, (int64_t)ch * nlast * 16) || !expect(k + 1, nlast))
       return fail(VFI_E_INVALID, "lastconv tensor sizes do not match this RIFE arch");
-    if ((r = build_lastconv(c, c->layers[b][10], ch, nlast, T[k], T[k + 1]))) return r;
-    if (arch == 426 && b + 1 < nb && (r = build_lastfeat(c, c->layers[b][11], ch, nlast, T[k], T[k + 1]))) return r;
+    // lastconv: column n = c5*16 + py*4 + px holds channel c5 < 5 at sub-pixel (py, px) of the cell's 4x4 patch
+    const auto flow_col = [](int n) { return shuffled(n >> 4, (n >> 2) & 3, n & 3); };
+    if ((r = build_layer(c, Lb[LAYER_LASTCONV], LAYER_LASTCONV, ch, 80,
+                         conv_transpose(T[k], T[k + 1], ch, nlast, flow_col))))
+      return r;
+    // arch 4.26: channels 5..12 (rife_arch.py:230-233, :272), the 8 features handed to the next block: column
+    // n = (py*4 + px)*8 + f, so 16 consecutive columns are two x-adjacent sub-pixels x 8 channels = 32 contiguous bytes
+    // of the [B, 4H, 4W, 8] output (out_s2d = 2)
+    const auto feat_col = [](int n) { return shuffled(5 + (n & 7), n >> 5, (n >> 3) & 3); };
+    if (block_has_layer(arch, b, LAYER_LASTFEAT) &&
+        (r = build_layer(c, Lb[LAYER_LASTFEAT], LAYER_LASTFEAT, ch, 128,
+                         conv_transpose(T[k], T[k + 1], ch, nlast, feat_col))))
+      return r;
     k += 2;
   }
+  // Head cnn1, cnn2 (3x3 + LeakyReLU) and cnn3 (ConvTranspose2d(creal, cout, 4, 2, 1)) of arch 4.17 / 4.26 from their
+  // weights and biases H[0..5], as tapconv layers on 32 channels, the kernel's smallest k-block (4.26's 16-channel layers
+  // zero-padded).  cnn3's column n = (a*2 + b)*cout + oc: its NHWC output [Hh][Wh][4*cout] IS the space-to-depth form of
+  // the feature map.
+  auto build_head = [&](const float* const* H, int creal, int cout) {
+    const auto col = [cout](int n) { return ConvTCol{n % cout, n / cout >> 1, n / cout & 1}; };
+    int r;
+    if ((r = build_layer(c, c->head[0], LAYER_HEAD_CONV, 32, 32, conv2d(H[0], H[1], creal, creal))) ||
+        (r = build_layer(c, c->head[1], LAYER_HEAD_CONV, 32, 32, conv2d(H[2], H[3], creal, creal))))
+      return r;
+    return build_layer(c, c->head[2], LAYER_HEAD_DECONV, 32, 4 * cout, conv_transpose(H[4], H[5], creal, cout, col));
+  };
   if (arch == 47) {  // encode = Conv2d(3,16,3,2,1) + ConvTranspose2d(16,4,4,2,1), fp32 on the CUDA cores
     const int64_t want[4] = {16 * 3 * 9, 16, 16 * 4 * 16, 4};
     for (int i = 0; i < 4; ++i) {
@@ -835,17 +756,13 @@ int vfi_rife_load(vfi_ctx* c, int arch, const float* const* T, const int64_t* nu
       std::vector<float> h(T[k + i], T[k + i] + want[i]);
       if ((r = upload(c, h, (void**)&c->enc[i]))) return r;
     }
-    if ((r = build_conv3x3_lrelu(c, c->head[0], 32, 32, T[k + 2], T[k + 3]))) return r;
-    if ((r = build_conv3x3_lrelu(c, c->head[1], 32, 32, T[k + 4], T[k + 5]))) return r;
-    if ((r = build_deconv_s2d(c, c->head[2], 32, 32, 8, T[k + 6], T[k + 7]))) return r;
-    for (int i = 0; i < 3; ++i)
-      if (c->head[i].nsplit < 1) return fail(VFI_E_STATE, "a head layer has no shared-memory plan");
+    if ((r = build_head(T + k + 2, 32, 8))) return r;
     k += 8;
   }
   if (arch == 426) {
     // encode = Head (rife_arch.py:378-395): the 16-channel layers run zero-padded to 32 channels - cnn0 on the CUDA
     // cores (fp32 weights, outputs 16..31 have zero weights and bias), cnn1..cnn3 as tapconv layers; cnn3's 4 output
-    // channels x 2x2 sub-pixels = 16 columns = the space-to-depth form of the 4-channel feature map
+    // channels x 2x2 sub-pixels = 16 columns
     const int64_t want[8] = {16 * 3 * 9, 16, 16 * 16 * 9, 16, 16 * 16 * 9, 16, 16 * 4 * 16, 4};
     for (int i = 0; i < 8; ++i)
       if (numel[k + i] != want[i]) return fail(VFI_E_INVALID, "encode tensor sizes do not match RIFE 4.26");
@@ -855,16 +772,9 @@ int vfi_rife_load(vfi_ctx* c, int arch, const float* const* T, const int64_t* nu
     std::copy(T[k + 1], T[k + 1] + 16, b0.begin());
     if ((r = upload(c, w0, (void**)&c->enc[0]))) return r;
     if ((r = upload(c, b0, (void**)&c->enc[1]))) return r;
-    if ((r = build_conv3x3_lrelu(c, c->head[0], 32, 16, T[k + 2], T[k + 3]))) return r;
-    if ((r = build_conv3x3_lrelu(c, c->head[1], 32, 16, T[k + 4], T[k + 5]))) return r;
-    if ((r = build_deconv_s2d(c, c->head[2], 32, 16, 4, T[k + 6], T[k + 7]))) return r;
-    for (int i = 0; i < 3; ++i)
-      if (c->head[i].nsplit < 1) return fail(VFI_E_STATE, "a head layer has no shared-memory plan");
+    if ((r = build_head(T + k + 2, 16, 4))) return r;
     k += 8;
   }
-  for (int b = 0; b < nb; ++b)
-    for (int l = 0; l < (arch == 426 && b + 1 < nb ? 12 : 11); ++l)
-      if (c->layers[b][l].nsplit < 1) return fail(VFI_E_STATE, "a layer has no shared-memory plan");
   c->loaded = true;
   return VFI_OK;
 }
@@ -1398,13 +1308,12 @@ int vfi_rife46_debug_layer(vfi_ctx* c, int block, int layer, const void* in, voi
                            int W, int impl, void* stream) {
   if (!c || block < 0 || layer < 0 || !in || !out) return fail(VFI_E_INVALID, "bad argument");
   if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
-  if (block >= num_blocks(c->arch) || layer > 11 || (layer == 11 && (c->arch != 426 || block + 1 >= num_blocks(c->arch))))
-    return fail(VFI_E_INVALID, "no such block / layer in the loaded arch");
+  if (!block_has_layer(c->arch, block, layer)) return fail(VFI_E_INVALID, "no such block / layer in the loaded arch");
   if (impl != TAPCONV_PLANNED && impl != TAPCONV_CHECKER && impl != TAPCONV_CELL_MAJOR)
     return fail(VFI_E_INVALID, "impl must be 0 (tensor cores), 1 (checker) or 2 (tensor cores, cell-major MMAs)");
   CK(cudaSetDevice(c->device));
   const TapConvLayer& L = c->layers[block][layer];
-  if (layer == 10) {
+  if (layer == LAYER_LASTCONV) {
     if (!out_mask) return fail(VFI_E_INVALID, "lastconv needs out_mask");
     LAUNCH(launch_tapconv(L, c->op_type, in, nullptr, (float4*)out, (float*)out_mask, B, H, W, c->num_sms, impl,
                           (cudaStream_t)stream));
@@ -1445,8 +1354,7 @@ int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_
                           int64_t* macs_per_cell, int* cmajor, int* wstream) {
   if (!c || block < 0 || layer < 0) return fail(VFI_E_INVALID, "bad argument");
   if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
-  if (block >= num_blocks(c->arch) || layer > 11 || (layer == 11 && (c->arch != 426 || block + 1 >= num_blocks(c->arch))))
-    return fail(VFI_E_INVALID, "no such block / layer in the loaded arch");
+  if (!block_has_layer(c->arch, block, layer)) return fail(VFI_E_INVALID, "no such block / layer in the loaded arch");
   const TapConvLayer& L = c->layers[block][layer];
   TapConvParams p{};
   const int st = tapconv_plan(L, &p);
@@ -1454,8 +1362,8 @@ int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_
   if (n_cta) *n_cta = L.n_cta;
   if (nsplit) *nsplit = L.nsplit;
   if (smem_bytes) *smem_bytes = (int)p.smem_bytes;
-  // (a streamed c = 96 ResConv issues two more K=16 steps with zero weights than its 9 x 96 products per output)
-  if (macs_per_cell) *macs_per_cell = (int64_t)(L.epi_mode == EPI_RESCONV ? 9 * L.cin : L.ktotal16 * 16) * L.n_total;
+  // (a streamed 3x3 layer may issue K=16 steps with zero weights after its 9 x cin products per output: c = 96 two)
+  if (macs_per_cell) *macs_per_cell = (int64_t)(L.wstream ? 9 * L.cin : L.ktotal16 * 16) * L.n_total;
   if (cmajor) *cmajor = p.cmajor;
   if (wstream) *wstream = p.wstream;
   return VFI_OK;

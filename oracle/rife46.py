@@ -187,7 +187,7 @@ def resconv(x, w, b, beta):
 
 
 def resconv_packed(sd: Dict[str, torch.Tensor], q: str, dt):
-    """The library's ResConv operands (csrc/rife46.cu build_resconv): (conv(x)+b)*beta == conv_{w*beta}(x) + b*beta, the
+    """The library's ResConv operands (csrc/rife46.cu conv2d with beta): (conv(x)+b)*beta == conv_{w*beta}(x) + b*beta, the
     products w*beta and b*beta formed in fp32, w*beta rounded to ``dt``; returned in float64."""
     beta = sd[q + "beta"].reshape(-1)
     return q16(sd[q + "conv.weight"] * beta.view(-1, 1, 1, 1), dt).double(), (sd[q + "conv.bias"] * beta).double()

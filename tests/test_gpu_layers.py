@@ -2,7 +2,7 @@
 
 Bounds: the tensor-core kernels take 16-bit operands (fp16 or bf16) and accumulate in fp32.  The reference y^ is the same
 operator in float64 on the SAME 16-bit inputs and the SAME packed weights as the library (round_T(w); ResConv:
-round_T(w*beta) with the shift b*beta, csrc/rife46.cu build_resconv), so only accumulation order and the output store
+round_T(w*beta) with the shift b*beta, csrc/rife46.cu conv2d with beta), so only accumulation order and the output store
 differ.  With K products per output and S = conv(|x|, |w|) + |shift| + |residual|, every element satisfies
     16-bit outputs:  |y - y^| <= ulp_T(y^) + 2 K 2^-24 S
     fp32 outputs:    |y - y^| <= 2 K 2^-24 S
