@@ -18,7 +18,7 @@ SYMBOLS = [
     "vfi_flavr_load", "vfi_flavr_forward", "vfi_flavr_debug_set_ref", "vfi_flavr_debug_conv", "vfi_flavr_layer_plan",
     "vfi_flavr_info",
     "vfi_ifrnet_load", "vfi_ifrnet_forward", "vfi_ifrnet_geometry", "vfi_ifrnet_debug_set_ref", "vfi_ifrnet_debug_conv",
-    "vfi_ifrnet_layer_plan", "vfi_ifrnet_info",
+    "vfi_ifrnet_layer_plan", "vfi_ifrnet_info", "vfi_streamconv_debug_conv", "vfi_streamconv_plan",
     # GMFSS building blocks (argtypes are set by gmfss.Ops)
     "vfi_gm_conv2d", "vfi_gm_conv2d_packed", "vfi_gm_transpose", "vfi_gm_convt4", "vfi_gm_instance_norm", "vfi_gm_layer_norm", "vfi_gm_softmax_rows", "vfi_gm_gemm", "vfi_gm_window", "vfi_gm_nchw_tokens", "vfi_gm_add_position", "vfi_gm_local_match", "vfi_gm_local_prop", "vfi_gm_convex_up", "vfi_gm_warp_zeros", "vfi_gm_resize", "vfi_gm_metric_input", "vfi_gm_pixel_shuffle2", "vfi_gm_axpby", "vfi_gm_copy_slice",
 ]
@@ -93,6 +93,9 @@ def lib():
     L.vfi_ifrnet_debug_conv.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp]
     L.vfi_ifrnet_layer_plan.argtypes = [vp, i32, vp, i32]
     L.vfi_ifrnet_info.argtypes = [vp, C.POINTER(i32)]
+    L.vfi_streamconv_debug_conv.argtypes = [vp, i32, f32, i32, vp, vp, vp, vp, i32, vp, i32, vp, i32, vp, vp, i32, i32, i32,
+                                            i32, i32, i32, vp]
+    L.vfi_streamconv_plan.argtypes = [vp, i32, vp, i32]
     for name in SYMBOLS:
         if name not in ("vfi_last_error", "vfi_version", "vfi_launch_count", "vfi_film_last_macs"):
             getattr(L, name).restype = i32

@@ -31,6 +31,7 @@
 #include <cstring>
 #include <type_traits>
 
+#include "../../include/vfi_b200.h"
 #include "ptx.cuh"
 #include "vfi_internal.h"
 
@@ -617,4 +618,105 @@ cudaError_t launch_streamconv(const StreamConvLayer& L, int op_type, const void*
 #endif  // VFI_HOST_EMU
 }
 
+namespace {
+// spec = {ksize, c0, c1, n_total, act, ext, n_f32, pad_before, pad_before_x, kt, pad_t, T_in, T_out}
+constexpr int kSpecLen = 13;
+bool layer_from_spec(const int32_t* spec, int n_spec, StreamConvLayer* L) {
+  if (!spec || n_spec != kSpecLen) return false;
+  L->ksize = spec[0];
+  L->c0 = spec[1];
+  L->c1 = spec[2];
+  L->n_total = spec[3];
+  L->act = spec[4];
+  L->ext = spec[5];
+  L->n_f32 = spec[6];
+  L->pad_before = spec[7];
+  L->pad_before_x = spec[8];
+  L->kt = spec[9];
+  L->pad_t = spec[10];
+  L->T_in = spec[11];
+  L->T_out = spec[12];
+  return true;
+}
+int sc_fail(int code, const std::string& msg) {
+  set_error(msg);
+  return code;
+}
+}  // namespace
+
 }  // namespace vfi
+
+using namespace vfi;
+
+extern "C" {
+
+/* Test hook: one streamconv layer from a plain description, packed by the product packer and run by the product launcher;
+ * no model context.  Weights, shift and slopes are HOST fp32; everything else lives on the device. */
+int vfi_streamconv_debug_conv(const int32_t* spec, int n_spec, float slope, int operand_type, const float* w,
+                              const float* shift, const float* slopes, const void* src0, int pitch0, const void* src1,
+                              int pitch1, void* out, int out_pitch, const void* res, float* out_f32, int f32_pitch, int B,
+                              int H, int W, int num_sms, int impl, void* stream) {
+  StreamConvLayer L;
+  if (!layer_from_spec(spec, n_spec, &L)) return sc_fail(VFI_E_INVALID, "streamconv: spec needs 13 values");
+  if (!w || !shift) return sc_fail(VFI_E_INVALID, "null argument");
+  if (operand_type != VFI_OPERAND_F16 && operand_type != VFI_OPERAND_BF16) return sc_fail(VFI_E_INVALID, "operand type");
+  if (impl != 0 && impl != 1) return sc_fail(VFI_E_INVALID, "streamconv: impl must be 0 (wgmma) or 1 (checker)");
+  L.slope = slope;
+  const int cin = L.c0 + L.c1, ntaps = L.ksize * L.ksize;
+  std::vector<uint16_t> pk;
+  StreamConvParams p{};
+  // w: logical [n_total][kt][ksize * ksize][c0 + c1]
+  if (!pack_streamconv3d(L, operand_type, [&](int n, int dt, int tap, int j) {
+        return w[(((size_t)n * L.kt + dt) * ntaps + tap) * cin + j];
+      }, &pk, &p))
+    return sc_fail(VFI_E_INVALID, "streamconv: unsupported layer shape");
+  int dev = 0;
+  if (num_sms <= 0) {
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+      return sc_fail(VFI_E_CUDA, "streamconv: no device");
+  }
+  void *dw = nullptr, *dshift = nullptr, *dslopes = nullptr;
+  cudaError_t e = cudaMalloc(&dw, pk.size() * 2);
+  if (e == cudaSuccess) e = cudaMalloc(&dshift, (size_t)L.n_total * 4);
+  if (e == cudaSuccess && slopes) e = cudaMalloc(&dslopes, (size_t)L.n_total * 4);
+  // the uploads go on the launch's stream, so the kernel reads them complete whatever kind of stream the caller passes
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dw, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dshift, shift, (size_t)L.n_total * 4, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess && slopes) e = cudaMemcpyAsync(dslopes, slopes, (size_t)L.n_total * 4, cudaMemcpyHostToDevice, st);
+  std::string what = "upload";
+  if (e == cudaSuccess) {
+    L.w = dw;
+    L.shift = static_cast<float*>(dshift);
+    L.slopes = static_cast<const float*>(dslopes);
+    set_error("");  // so that only a message the launcher sets now is reported with its error
+    e = launch_streamconv(L, operand_type, src0, pitch0, src1, pitch1, out, out_pitch, B, H, W, num_sms, impl == 1, st, res,
+                          out_f32, f32_pitch);
+    const std::string msg = vfi_last_error();
+    what = msg.empty() ? "launch" : "launch: " + msg;
+  }
+  // the uploads and the run finish before the buffers are freed (and pk goes out of scope)
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e == cudaSuccess && es != cudaSuccess) {
+    e = es;
+    what = "run";
+  }
+  cudaFree(dw);
+  cudaFree(dshift);
+  cudaFree(dslopes);
+  if (e != cudaSuccess) return sc_fail(VFI_E_CUDA, "streamconv: " + what + ": " + cudaGetErrorString(e));
+  return VFI_OK;
+}
+
+/* Test hook: the plan of a layer {n_cta, nsplit, a_slots, b_slots, smem_bytes, halo_y0, halo_x0}, or its refusal. */
+int vfi_streamconv_plan(const int32_t* spec, int n_spec, int32_t* info, int cap) {
+  StreamConvLayer L;
+  if (!layer_from_spec(spec, n_spec, &L) || !info) return sc_fail(VFI_E_INVALID, "streamconv: spec needs 13 values");
+  StreamConvParams p{};
+  if (!streamconv_plan(L, &p)) return sc_fail(VFI_E_INVALID, "streamconv: unsupported layer shape");
+  const int32_t v[7] = {p.n_cta, p.nsplit, p.a_slots, p.b_slots, (int32_t)p.smem_bytes, p.halo_y0, p.halo_x0};
+  for (int i = 0; i < cap && i < 7; ++i) info[i] = v[i];
+  return VFI_OK;
+}
+
+}  // extern "C"

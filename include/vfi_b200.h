@@ -249,6 +249,21 @@ int vfi_rife46_debug_state(vfi_ctx* ctx, float* flow4_out, float* mask_out, int 
 int vfi_rife46_layer_plan(vfi_ctx* ctx, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
                           int64_t* macs_per_cell, int* cmajor, int* wstream);
 int vfi_sync(vfi_ctx* ctx);
+/* Run ONE streamconv layer (csrc/streamconv.cu, the conv kernel of FILM, Sepconv, FLAVR and IFRNet) from a plain
+ * description, without a model: spec = {ksize, c0, c1, n_total, act, ext, n_f32, pad_before, pad_before_x, kt, pad_t,
+ * T_in, T_out} (the fields of the layer; n_spec = 13), slope = the ext 1 PReLU slope.  HOST fp32: w [n_total][kt]
+ * [ksize * ksize][c0 + c1], shift [n_total], slopes [n_total] (ext 2; may be NULL otherwise); they are packed by the
+ * product packer into temporary device buffers.  DEVICE: the 16-bit NHWC source / output / residual slices (pointer +
+ * pixel pitch in elements; B samples of T_in / T_out planes) and the fp32 slice of the first n_f32 columns.
+ * num_sms <= 0: the device's SM count (a smaller value makes every CTA walk more passes).  impl 0 = wgmma kernel,
+ * 1 = CUDA-core checker.  Synchronises `stream`; returns the launch's or the run's error. */
+int vfi_streamconv_debug_conv(const int32_t* spec, int n_spec, float slope, int operand_type, const float* w,
+                              const float* shift, const float* slopes, const void* src0, int pitch0, const void* src1,
+                              int pitch1, void* out, int out_pitch, const void* res, float* out_f32, int f32_pitch, int B,
+                              int H, int W, int num_sms, int impl, void* stream);
+/* The plan of such a layer: {n_cta, nsplit, a_slots, b_slots, smem_bytes, halo_y0, halo_x0}, or VFI_E_INVALID when
+ * streamconv cannot run it.  No GPU needed. */
+int vfi_streamconv_plan(const int32_t* spec, int n_spec, int32_t* info, int cap);
 
 /* Measurement hook (bench.py's roofline lines): while enabled, every internal pass of the RIFE forward schedule records
  * CUDA events on its launching stream around each kernel group - id = 10 * block + {0 front (warps + resample + concat,

@@ -85,7 +85,11 @@ static inline cudaError_t emu_memset_async(void* d, int v, size_t n, cudaStream_
 #define cudaMalloc(p, n) emu_malloc((void**)(p), (n))
 #define cudaFree(p) emu_free(p)
 #define cudaMemcpy(d, s, n, k) emu_memcpy((d), (s), (n), (k))
+#define cudaMemcpyAsync(d, s, n, k, st) emu_memcpy((d), (s), (n), (k))
 #define cudaMemsetAsync(d, v, n, st) emu_memset_async((d), (v), (n), (st))
 #define cudaSetDevice(d) cudaSuccess
 #define cudaGetLastError() cudaSuccess
 #define cudaGetErrorString(e) "emulated CUDA error"
+#define cudaGetDevice(p) (*(p) = 0, cudaSuccess)
+#define cudaDeviceGetAttribute(v, a, d) (*(v) = 132, cudaSuccess)
+#define cudaStreamSynchronize(s) cudaSuccess

@@ -121,6 +121,8 @@ static inline cudaError_t emu_memcpy(void* d, const void* s, size_t n) {
 #define cudaGetDeviceProperties(p, d) emu_props((p), (d))
 #define cudaDeviceSynchronize() cudaSuccess
 #define cudaStreamSynchronize(s) cudaSuccess
+#define cudaGetDevice(p) (*(p) = 0, cudaSuccess)
+#define cudaDeviceGetAttribute(v, a, d) (*(v) = 132, cudaSuccess)
 #define cudaStreamCreateWithFlags(p, f) (*(p) = nullptr, cudaSuccess)
 #define cudaStreamDestroy(s) cudaSuccess
 #define cudaStreamWaitEvent(s, e, f) cudaSuccess
