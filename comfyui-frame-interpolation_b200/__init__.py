@@ -1,4 +1,4 @@
-"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR, IFRNet) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
+"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR, IFRNet, CAIN) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
 
 Exports the same mapping names ComfyUI discovers in the reference's root __init__.py:23-47.
 """
@@ -8,6 +8,7 @@ from .sepconv_node import SepconvVFI  # noqa: F401
 from .gmfss_node import GMFSS_Fortuna_VFI  # noqa: F401
 from .flavr_node import FLAVR_VFI  # noqa: F401
 from .ifrnet_node import IFRNet_VFI  # noqa: F401
+from .cain_node import CAIN_VFI  # noqa: F401
 
 NODE_CLASS_MAPPINGS = {
     "RIFE VFI": RIFE_VFI,
@@ -16,6 +17,7 @@ NODE_CLASS_MAPPINGS = {
     "GMFSS Fortuna VFI": GMFSS_Fortuna_VFI,
     "FLAVR VFI": FLAVR_VFI,
     "IFRNet VFI": IFRNet_VFI,
+    "CAIN VFI": CAIN_VFI,
     "Make Interpolation State List": MakeInterpolationStateList,
     "VFI FloatToInt": FloatToInt,
 }
@@ -27,4 +29,5 @@ NODE_DISPLAY_NAME_MAPPINGS = {
     "GMFSS Fortuna VFI": "GMFSS Fortuna VFI (H100 native)",
     "FLAVR VFI": "FLAVR VFI (H100 native)",
     "IFRNet VFI": "IFRNet VFI (H100 native)",
+    "CAIN VFI": "CAIN VFI (H100 native)",
 }

@@ -205,6 +205,7 @@ struct vfi_ctx {
   vfi::SepState* sep = nullptr;    // Sepconv weights and workspace (sepconv.cu)
   vfi::ModelState* flavr = nullptr;  // FLAVR weights and workspace (flavr.cu)
   vfi::ModelState* ifrnet = nullptr;  // IFRNet weights and workspace (ifrnet.cu)
+  vfi::ModelState* cain = nullptr;    // CAIN weights and workspace (cain.cu)
 };
 
 namespace vfi {
@@ -213,6 +214,7 @@ FilmState*& ctx_film(::vfi_ctx* c) { return c->film; }
 SepState*& ctx_sep(::vfi_ctx* c) { return c->sep; }
 ModelState*& ctx_flavr(::vfi_ctx* c) { return c->flavr; }
 ModelState*& ctx_ifrnet(::vfi_ctx* c) { return c->ifrnet; }
+ModelState*& ctx_cain(::vfi_ctx* c) { return c->cain; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi
 
@@ -584,6 +586,8 @@ int vfi_destroy(vfi_ctx* c) {
   c->flavr = nullptr;
   delete c->ifrnet;
   c->ifrnet = nullptr;
+  delete c->cain;
+  c->cain = nullptr;
   c->film = nullptr;
   sepconv_destroy(c->sep);
   c->sep = nullptr;

@@ -321,6 +321,23 @@ cudaError_t launch_ifrnet_final(const float* f0, const float* f1, int H, int W, 
                                 int wq, int hF, int wF, float scale, float fmul, const float* mean, float* out,
                                 cudaStream_t st);
 
+// ---- CAIN kernels around the convolutions (cain_elem.cu); 16-bit tensors on the bordered (h + 2) x (w + 2) grid,
+// 192 channels per cell (the prep output 384); frames and output are fp32 [3][H][W] planes ----
+constexpr int kCainChannels = 192;   // trunk channels (3 x 4^3)
+constexpr int kCainMeanChunks = 64;  // partial sums per frame plane (doubles: 6 x kCainMeanChunks)
+constexpr int kCainHidden = 12;      // CALayer's 192 / 16
+cudaError_t launch_cain_frame_sums(const float* f0, const float* f1, int H, int W, double* partial, cudaStream_t st);
+cudaError_t launch_cain_prep(int op, const float* f0, const float* f1, int H, int W, int top, int left, int h, int w,
+                             const double* partial, void* out, cudaStream_t st);
+// reflect: border = ReflectionPad2d(1) of the interior (add must be null); else border = 0 and interior += add (if any)
+cudaError_t launch_cain_border(int op, void* x, const void* add, int h, int w, bool reflect, cudaStream_t st);
+cudaError_t launch_cain_chan_sums(int op, const void* x, int h, int w, float* partial, cudaStream_t st);  // [h][192]
+cudaError_t launch_cain_gate(const float* partial, int h, int w, const float* ca, float* g, cudaStream_t st);
+cudaError_t launch_cain_apply(int op, const void* x, const float* g, const void* res, void* out, int h, int w,
+                              cudaStream_t st);
+cudaError_t launch_cain_final(int op, const void* feat, int H, int W, int top, int left, int w, const double* partial,
+                              float* out, cudaStream_t st);
+
 cudaError_t launch_adacof(const float* in, const float* weight, const float* off_i, const float* off_j, float* out, int N,
                           int C, int Hin, int Win, int F, int dil, int Ho, int Wo, cudaStream_t st);
 cudaError_t launch_edt_pass(const float* data, float* out, int bs, int h, int w, float diam2, cudaStream_t st);
@@ -344,6 +361,7 @@ CtxInfo ctx_info(::vfi_ctx* c);
 FilmState*& ctx_film(::vfi_ctx* c);
 ModelState*& ctx_flavr(::vfi_ctx* c);  // a FlavrState (flavr.cu)
 ModelState*& ctx_ifrnet(::vfi_ctx* c);  // an IfrnetState (ifrnet.cu)
+ModelState*& ctx_cain(::vfi_ctx* c);    // a CainState (cain.cu)
 SepState*& ctx_sep(::vfi_ctx* c);
 void ctx_add_launches(::vfi_ctx* c, int n);
 

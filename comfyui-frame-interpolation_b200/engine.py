@@ -621,3 +621,112 @@ class IfrnetEngine:
 
     def sync(self):
         check(self._L.vfi_sync(self._ctx))
+
+
+# CAIN(depth=3).state_dict(): Interpolation(5, 12, 192) - headConv, 5 groups of 12 RCABs (conv1, conv2, CALayer
+# 192 -> 12 -> 192) and a tail conv, tailConv (cain_arch.py, common.py)
+def cain_state_dict_spec():
+    """CAIN(depth=3).state_dict() names and shapes, in order (494 tensors)."""
+    C_, R, pre = 192, 12, "encoder.interpolate."
+    spec = [(pre + "headConv.weight", (C_, 2 * C_, 3, 3)), (pre + "headConv.bias", (C_,))]
+    for g in range(5):
+        for r in range(12):
+            p = f"{pre}body.{g}.body.{r}.body."
+            spec += [(p + "0.conv.weight", (C_, C_, 3, 3)), (p + "0.conv.bias", (C_,)),
+                     (p + "2.conv.weight", (C_, C_, 3, 3)), (p + "2.conv.bias", (C_,)),
+                     (p + "3.conv_du.0.weight", (R, C_, 1, 1)), (p + "3.conv_du.0.bias", (R,)),
+                     (p + "3.conv_du.2.weight", (C_, R, 1, 1)), (p + "3.conv_du.2.bias", (C_,))]
+        spec += [(f"{pre}body.{g}.body.12.conv.weight", (C_, C_, 3, 3)), (f"{pre}body.{g}.body.12.conv.bias", (C_,))]
+    spec += [(pre + "tailConv.weight", (C_, C_, 3, 3)), (pre + "tailConv.bias", (C_,))]
+    return spec
+
+
+def cain_geometry(h: int, w: int):
+    """The sizes vfi_cain_forward uses for an h x w frame: padded size, trunk grid, padding before; raises VfiError for
+    a frame the reference's ReflectionPad2d cannot pad."""
+    v = np.zeros(6, np.int32)
+    check(lib().vfi_cain_geometry(int(h), int(w), v.ctypes.data, 6))
+    return dict(zip(("hp", "wp", "gh", "gw", "top", "left"), [int(x) for x in v]))
+
+
+class CainEngine:
+    """CAIN (pretrained_cain.pth, CAIN(depth=3)) on one H100: `state_dict` = CAIN's, without the checkpoint's "module."
+    prefix; every name and shape is checked.  fp16 operands with fp32 accumulation ("float32", as the node runs it); the
+    means, the attention gates and the output are fp32."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, dtype: str = "float32"):
+        if not torch.cuda.is_available():
+            raise VfiError("no CUDA device: this path has no CPU fallback")
+        if dtype not in OPERAND:
+            raise ValueError(f"dtype must be one of {list(OPERAND)}")
+        spec = cain_state_dict_spec()
+        for name, shape in spec:
+            if name not in state_dict:
+                raise KeyError(f"state_dict is not a CAIN checkpoint; missing {name}")
+            if tuple(state_dict[name].shape) != shape:
+                raise ValueError(f"CAIN: {name} has shape {tuple(state_dict[name].shape)}, expected {shape}")
+        self._L = lib()
+        self.device = int(device)
+        self._ctx = C.c_void_p()
+        check(self._L.vfi_create(self.device, C.byref(self._ctx)))
+        hold = [state_dict[n].detach().to("cpu", torch.float32).contiguous() for n, _ in spec]
+        ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+        numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+        check(self._L.vfi_cain_load(self._ctx, ptrs, numel, len(hold), OPERAND[dtype]))
+        self.dtype = dtype
+
+    def close(self):
+        if getattr(self, "_ctx", None) is not None and self._ctx.value:
+            self._L.vfi_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def forward(self, img0: torch.Tensor, img1: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """img0, img1: CUDA float32 [1, 3, H, W] -> [1, 3, H, W] = model(img0, img1)[0] (not clamped)."""
+        for x in (img0, img1):
+            assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4 and x.shape[:2] == (1, 3)
+        assert img0.shape == img1.shape
+        _, _, h, w = img0.shape
+        if out is None:
+            out = torch.empty((1, 3, h, w), dtype=torch.float32, device=img0.device)
+        assert out.is_cuda and out.is_contiguous() and out.dtype == torch.float32 and out.shape == img0.shape
+        st = torch.cuda.current_stream(img0.device).cuda_stream
+        check(self._L.vfi_cain_forward(self._ctx, img0.data_ptr(), img1.data_ptr(), h, w, out.data_ptr(), st))
+        return out
+
+    # ------------------------------------------------------------------ hooks
+    def set_ref(self, use_ref: bool):
+        check(self._L.vfi_cain_debug_set_ref(self._ctx, 1 if use_ref else 0))
+
+    def debug_conv(self, layer, src0, pitch0, src1, pitch1, out, out_pitch, n_images, H, W, impl=0, res=None):
+        """One conv layer on raw 16-bit NHWC tensors (pointers with element offsets already applied)."""
+        st = torch.cuda.current_stream(src0.device).cuda_stream
+        check(self._L.vfi_cain_debug_conv(
+            self._ctx, layer, src0.data_ptr(), int(pitch0), None if src1 is None else src1.data_ptr(), int(pitch1),
+            out.data_ptr(), int(out_pitch), None if res is None else res.data_ptr(), n_images, H, W, impl, st))
+        return out
+
+    def layer_plan(self, layer):
+        v = np.zeros(11, np.int32)
+        check(self._L.vfi_cain_layer_plan(self._ctx, layer, v.ctypes.data, 11))
+        keys = ("c0", "c1", "n_total", "ksize", "act", "ext", "n_cta", "nsplit", "a_slots", "b_slots", "smem_bytes")
+        return dict(zip(keys, [int(x) for x in v]))
+
+    def debug_elem(self, kernel, H, W, img0=None, img1=None, x=None, res=None, out=None, rcab=0):
+        """One element-wise stage for an H x W frame (vfi_cain_debug_elem): 0 prep, 1 reflected border, 2 zero border
+        + res, 3 channel attention of RCAB `rcab`, 4 final."""
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        check(self._L.vfi_cain_debug_elem(self._ctx, kernel, p(img0), p(img1), H, W, p(x), p(res), p(out), rcab, st))
+        return out
+
+    def launch_count(self) -> int:
+        return int(self._L.vfi_launch_count(self._ctx))
+
+    def sync(self):
+        check(self._L.vfi_sync(self._ctx))

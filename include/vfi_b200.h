@@ -231,6 +231,34 @@ int vfi_ifrnet_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0,
 int vfi_ifrnet_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
 int vfi_ifrnet_info(vfi_ctx* ctx, int* variant);
 
+/* CAIN (`CAIN VFI` node: CAIN(depth=3)) ---------------------------------------------------------------------- */
+#define VFI_CAIN_NUM_TENSORS 494
+/* Replaces: CAIN(depth=3).load_state_dict(sd) with the checkpoint's "module." prefix stripped (cain/__init__.py:
+ * 42-48).  HOST float32 arrays in state_dict() order (engine.py cain_state_dict_spec); every tensor's size is checked and
+ * a refusal names the tensor. */
+int vfi_cain_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type);
+/* Replaces: `model(img0, img1)[0]` for one pair (CAIN.forward, cain_arch.py).  DEVICE pointers: img0, img1 and out are
+ * float32 [3][H][W] planes (NCHW, batch 1); out is not clamped.  A frame the reference's ReflectionPad2d cannot pad
+ * (padding on a side not smaller than the axis) is refused before any launch.  Asynchronous on `stream`. */
+int vfi_cain_forward(vfi_ctx* ctx, const float* img0, const float* img1, int H, int W, float* out, void* stream);
+/* The sizes vfi_cain_forward would use (no context): {Hp, Wp, trunk grid h, w, padding top, left} (6 values), or the
+ * error it would return. */
+int vfi_cain_geometry(int H, int W, int32_t* info, int cap);
+/* Test hooks: every conv through the CUDA-core checker (1) / the wgmma kernel (0); run one conv layer (id: 0 headConv,
+ * 1 + 25 g + 2 r + {0 conv1, 1 conv2} of RCAB r in group g, 1 + 25 g + 24 the group's tail conv, 126 tailConv) on
+ * 16-bit NHWC slices; its plan {c0, c1, n_total, ksize, act, ext, n_cta, nsplit, a_slots, b_slots, smem_bytes}.
+ * vfi_cain_debug_elem runs one element-wise stage for an H x W frame on DEVICE tensors of the bordered grid
+ * ((h + 2) x (w + 2) cells of 192 16-bit channels, h x w from vfi_cain_geometry): kernel 0 prep (img0, img1 -> out of
+ * 384 channels), 1 reflected border of out (in place), 2 zero border of out and res added to its interior, 3 channel
+ * attention of RCAB `rcab` (0..59): out = x * gate(mean of x's interior) + res on every cell, 4 final (x, with the
+ * means of img0 and img1 -> out float32 [3][H][W]).  Asynchronous on `stream`. */
+int vfi_cain_debug_set_ref(vfi_ctx* ctx, int use_ref);
+int vfi_cain_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0, const void* src1, int pitch1, void* out,
+                        int out_pitch, const void* res, int n_images, int H, int W, int impl, void* stream);
+int vfi_cain_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
+int vfi_cain_debug_elem(vfi_ctx* ctx, int kernel, const float* img0, const float* img1, int H, int W, const void* x,
+                        const void* res, void* out, int rcab, void* stream);
+
 /* Test / profiling hooks (used by tests/ and bench.py only) --------------------------------------------- */
 /* Run ONE convolution layer of block `block` (0..3; arch 4.26: 0..4): layer 0 = conv0.0, 1 = conv0.1, 2..9 = ResConv
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
@@ -249,7 +277,7 @@ int vfi_rife46_debug_state(vfi_ctx* ctx, float* flow4_out, float* mask_out, int 
 int vfi_rife46_layer_plan(vfi_ctx* ctx, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
                           int64_t* macs_per_cell, int* cmajor, int* wstream);
 int vfi_sync(vfi_ctx* ctx);
-/* Run ONE streamconv layer (csrc/streamconv.cu, the conv kernel of FILM, Sepconv, FLAVR and IFRNet) from a plain
+/* Run ONE streamconv layer (csrc/streamconv.cu, the conv kernel of FILM, Sepconv, FLAVR, IFRNet and CAIN) from a plain
  * description, without a model: spec = {ksize, c0, c1, n_total, act, ext, n_f32, pad_before, pad_before_x, kt, pad_t,
  * T_in, T_out} (the fields of the layer; n_spec = 13), slope = the ext 1 PReLU slope.  HOST fp32: w [n_total][kt]
  * [ksize * ksize][c0 + c1], shift [n_total], slopes [n_total] (ext 2; may be NULL otherwise); they are packed by the
