@@ -13,7 +13,7 @@ SYMBOLS = [
     "vfi_rife46_debug_layer", "vfi_rife46_debug_state", "vfi_rife46_layer_plan", "vfi_sync",
     "vfi_rife_profile", "vfi_rife_profile_read", "vfi_host_copy_frames",
     "vfi_film_load", "vfi_film_forward", "vfi_film_debug_set_ref", "vfi_film_debug_conv", "vfi_film_layer_plan",
-    "vfi_film_last_macs", "vfi_film_debug_pack_host",
+    "vfi_film_last_macs", "vfi_film_debug_pack_host", "vfi_film_debug_state", "vfi_film_debug_elem",
     "vfi_sepconv_load", "vfi_sepconv_forward", "vfi_sepconv_debug_set_ref", "vfi_sepconv_debug_pack_host",
     "vfi_flavr_load", "vfi_flavr_forward", "vfi_flavr_debug_set_ref", "vfi_flavr_debug_conv", "vfi_flavr_layer_plan",
     "vfi_flavr_info",
@@ -77,6 +77,9 @@ def lib():
     L.vfi_film_last_macs.argtypes = [vp]
     L.vfi_film_debug_pack_host.argtypes = [i32, i32, i32, i32, i32, i32, vp, i32, i32, vp, i64] + [C.POINTER(i32)] * 4
     L.vfi_film_last_macs.restype = i64
+    L.vfi_film_debug_state.argtypes = [vp, i32, i32, vp, i32, C.POINTER(i32), C.POINTER(i32)]
+    L.vfi_film_debug_elem.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, i32, i32,
+                                      vp]
     L.vfi_sepconv_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]
     L.vfi_sepconv_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, vp, vp]
     L.vfi_sepconv_debug_set_ref.argtypes = [vp, i32]

@@ -73,6 +73,8 @@ struct FilmState {
   Buf img[kLevels], feat[kLevels], v[2][kLevels], aligned[kFuseLevels];
   Buf tmpA, tmpB, vup, wb, t0, t1, t3, upbuf, n0, n1, n2;
   int64_t macs = 0;  // tensor-core MACs of the last forward (real channels, bench.py)
+  int last_B = 0;    // pairs and level sizes of the last forward (vfi_film_debug_state)
+  int last_H[kLevels] = {}, last_W[kLevels] = {};
 };
 
 void film_destroy(FilmState* f) {
@@ -268,6 +270,9 @@ int forward(vfi_ctx* c, FilmState* f, const float* frames, int n_frames, int H, 
     d.W[l] = d.W[l - 1] >> 1;
   }
   RUN(ensure_workspace(f, d, B));
+  f->last_B = B;
+  std::copy(d.H, d.H + kLevels, f->last_H);
+  std::copy(d.W, d.W + kLevels, f->last_W);
   Runner r{c, f, ctx_info(c), st};
   const int op = f->op_type;
   f->macs = 0;
@@ -486,6 +491,74 @@ int vfi_film_debug_conv(vfi_ctx* c, int group, int layer, const void* src0, int 
                                           ctx_info(c).num_sms, impl != 0, static_cast<cudaStream_t>(stream));
   ctx_add_launches(c, 1);
   if (e != cudaSuccess) return ffail(VFI_E_CUDA, std::string("streamconv: ") + cudaGetErrorString(e) + " / " + vfi_last_error());
+  return VFI_OK;
+}
+
+int vfi_film_debug_state(vfi_ctx* c, int dir, int level, float* out, int batch, int* H, int* W) {
+  FilmState* f = c ? ctx_film(c) : nullptr;
+  if (!f || !f->loaded) return ffail(VFI_E_STATE, "vfi_film_load has not been called");
+  if (!H || !W) return ffail(VFI_E_INVALID, "null argument");
+  if (dir < 0 || dir > 1 || level < 0 || level >= kLevels) return ffail(VFI_E_INVALID, "film: no such flow level");
+  if (!f->last_B) return ffail(VFI_E_STATE, "film: no forward has run");
+  FCK(cudaSetDevice(ctx_info(c).device));
+  FCK(cudaDeviceSynchronize());
+  *H = f->last_H[level];
+  *W = f->last_W[level];
+  if (!out) return VFI_OK;
+  if (batch < 1 || batch > f->last_B) return ffail(VFI_E_INVALID, "film: batch larger than the last forward");
+  FCK(cudaMemcpy(out, f->v[dir][level].p, (size_t)batch * *H * *W * 2 * sizeof(float), cudaMemcpyDeviceToDevice));
+  FCK(cudaDeviceSynchronize());
+  return VFI_OK;
+}
+
+int vfi_film_debug_elem(vfi_ctx* c, int kernel, const void* in0, int in_pitch, const void* in1, const void* in2,
+                        const void* in3, const int32_t* frame_idx, void* out, int out_pitch, int C, int B, int H, int W,
+                        int h, int w, float fscale, int clamp01, int predictor, void* stream) {
+  FilmState* f = c ? ctx_film(c) : nullptr;
+  if (!f || !f->loaded) return ffail(VFI_E_STATE, "vfi_film_load has not been called");
+  if (B < 1 || H < 1 || W < 1) return ffail(VFI_E_INVALID, "film: empty launch");
+  const int op = f->op_type;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  FCK(cudaSetDevice(ctx_info(c).device));
+  cudaError_t e = cudaSuccess;
+  switch (kernel) {
+    case 0: {
+      if (B > 2 * kMaxBatch || !frame_idx) return ffail(VFI_E_INVALID, "film: gather_rgb takes 1..32 frame indices");
+      FilmFrameIdx idx{};
+      for (int i = 0; i < B; ++i) idx.i[i] = frame_idx[i];
+      e = launch_film_gather_rgb((const float*)in0, C, idx, B, H, W, (float*)out, st);
+      break;
+    }
+    case 1: e = launch_film_pool_rgb((const float*)in0, (float*)out, B, H, W, st); break;
+    case 2: e = launch_film_conv_rgb(op, (const float*)in0, f->rgb_w, f->rgb_b, out, out_pitch, B, H, W, st); break;
+    case 3: e = launch_film_pool16(op, in0, in_pitch, out, out_pitch, C, B, H, W, st); break;
+    case 4: e = launch_film_flow_up((const float*)in0, h, w, (float*)out, B, H, W, st); break;
+    case 5: e = launch_film_warp16(op, in0, in_pitch, C, (const float*)in1, fscale, out, out_pitch, B, H, W, st); break;
+    case 6:
+      e = launch_film_misc64(op, (const float*)in0, (const float*)in1, (const float*)in2, (const float*)in3, out, out_pitch,
+                             B, H, W, st);
+      break;
+    case 7: e = launch_film_nearest16(in0, h, w, out, C, B, H, W, st); break;
+    case 8:
+      if (predictor < 0 || predictor > 3) return ffail(VFI_E_INVALID, "film: no such flow predictor");
+      if (C <= 128 && C != kFlowNF[predictor] / 2)
+        return ffail(VFI_E_INVALID, "film: flow_head of predictor " + std::to_string(predictor) + " reads " +
+                                        std::to_string(kFlowNF[predictor] / 2) + " channels");
+      e = launch_film_flow_head(op, in0, in_pitch, C, f->head_w[predictor], f->head_b[predictor], (const float*)in1,
+                                (float*)out, B, H, W, st);
+      break;
+    case 9: e = launch_film_out_rgb(op, in0, in_pitch, f->out_w, f->out_b, clamp01, (float*)out, B, H, W, st); break;
+    default: return ffail(VFI_E_INVALID, "film: no such element-wise kernel");
+  }
+  ctx_add_launches(c, 1);
+  if (e == cudaErrorInvalidValue) {  // the launchers' refusals, named
+    if ((kernel == 3 || kernel == 5 || kernel == 7 || kernel == 8) && (C & 7))
+      return ffail(VFI_E_INVALID, "film: C must be a multiple of 8");
+    if (kernel == 8) return ffail(VFI_E_INVALID, "film: flow_head reads at most 128 channels");
+    if (kernel == 1 || kernel == 3) return ffail(VFI_E_INVALID, "film: level too small to pool");
+    return ffail(VFI_E_INVALID, "film: launch refused");
+  }
+  if (e != cudaSuccess) return ffail(VFI_E_CUDA, std::string("film: element-wise launch: ") + cudaGetErrorString(e));
   return VFI_OK;
 }
 

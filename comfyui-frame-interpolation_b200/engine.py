@@ -287,6 +287,27 @@ class FilmEngine:
             out.data_ptr(), int(out_pitch if out_pitch is not None else out.shape[-1]), B, H, W, impl, st))
         return out
 
+    def debug_state(self, direction, level, batch):
+        """Flow v[direction][level] of the last forward (0 forward, 1 backward; level 0..6) as a CUDA float32
+        [batch, H_l, W_l, 2] tensor (vfi_film_debug_state)."""
+        h, w = C.c_int(), C.c_int()
+        check(self._L.vfi_film_debug_state(self._ctx, direction, level, None, batch, C.byref(h), C.byref(w)))
+        out = torch.empty((batch, h.value, w.value, 2), dtype=torch.float32, device=f"cuda:{self.device}")
+        check(self._L.vfi_film_debug_state(self._ctx, direction, level, out.data_ptr(), batch, C.byref(h), C.byref(w)))
+        return out
+
+    def debug_elem(self, kernel, in0, out, C_, B, H, W, in_pitch=0, in1=None, in2=None, in3=None, frame_idx=None,
+                   out_pitch=0, h=0, w=0, fscale=1.0, clamp01=False, predictor=0):
+        """One film_elem.cu kernel on CUDA tensors (vfi_film_debug_elem; kernel ids in include/vfi_b200.h).  in* and out
+        may be tensor views: their data_ptr() is the slice start, the pitches are in elements."""
+        p = lambda t: None if t is None else t.data_ptr()   # noqa: E731
+        idx = None if frame_idx is None else _i32(frame_idx)
+        st = torch.cuda.current_stream(in0.device).cuda_stream
+        check(self._L.vfi_film_debug_elem(self._ctx, kernel, p(in0), int(in_pitch), p(in1), p(in2), p(in3),
+                                          None if idx is None else idx.ctypes.data, p(out), int(out_pitch), int(C_), B, H,
+                                          W, h, w, float(fscale), 1 if clamp01 else 0, predictor, st))
+        return out
+
     def layer_plan(self, group, layer):
         v = [C.c_int() for _ in range(10)]
         check(self._L.vfi_film_layer_plan(self._ctx, group, layer, *[C.byref(x) for x in v]))

@@ -154,6 +154,25 @@ int vfi_film_debug_conv(vfi_ctx* ctx, int group, int layer, const void* src0, in
 int vfi_film_layer_plan(vfi_ctx* ctx, int group, int layer, int* c0, int* c1, int* n_total, int* ksize, int* n_cta,
                         int* nsplit, int* mt, int* a_slots, int* b_slots, int* smem_bytes);
 int64_t vfi_film_last_macs(const vfi_ctx* ctx);
+/* Test hooks.  vfi_film_debug_state copies the flow v[dir][level] of the last forward (dir 0 forward, 1 backward; level
+ * 0..6, [batch, H_l, W_l, 2] float32) into a caller DEVICE buffer and synchronises; `out` NULL only returns H_l, W_l.
+ * vfi_film_debug_elem runs one kernel of film_elem.cu on caller DEVICE tensors (16-bit slices: pointer + pixel pitch in
+ * elements) with the loaded operand type and weights; asynchronous on `stream`.  kernel:
+ *   0 gather_rgb  in0 frames [*, H, W, C] float32 -> out [B, H, W, 3]; frame_idx: HOST, B (<= 32) source frames
+ *   1 pool_rgb    in0 [B, H, W, 3] -> out [B, H/2, W/2, 3] float32
+ *   2 conv_rgb    in0 [B, H, W, 3] float32 -> out 64 channels (extract.convs.0.0 + LeakyReLU)
+ *   3 pool16      in0 C channels at H x W -> out at H/2 x W/2
+ *   4 flow_up     in0 flow [B, h, w, 2] -> out 2 * bilinear resize [B, H, W, 2] float32
+ *   5 warp16      in0 C channels, in1 flow [B, H, W, 2] float32 scaled by fscale -> out C channels
+ *   6 misc64      in0 / in1 images [B, H, W, 3], in2 backward / in3 forward flow -> out 64 channels
+ *   7 nearest16   in0 [B, h, w, C] -> out [B, H, W, C] (both packed)
+ *   8 flow_head   in0 C = nf/2 channels of predictor `predictor` (0..3), in1 up-sampled flow or NULL -> out flow float32
+ *   9 out_rgb     in0 64 channels -> out [B, H, W, 3] float32, clamped to [0, 1] if clamp01
+ * A launch the kernel's launcher refuses returns VFI_E_INVALID and names the reason. */
+int vfi_film_debug_state(vfi_ctx* ctx, int dir, int level, float* out, int batch, int* H, int* W);
+int vfi_film_debug_elem(vfi_ctx* ctx, int kernel, const void* in0, int in_pitch, const void* in1, const void* in2,
+                        const void* in3, const int32_t* frame_idx, void* out, int out_pitch, int C, int B, int H, int W,
+                        int h, int w, float fscale, int clamp01, int predictor, void* stream);
 /* Host-only: vfi_film_load's weight packer on caller data (layout 0 = reference channel order padded to 64; layout 1 = a
  * fusion level's [wfeat0 C | wfeat1 C | misc 64] + nf decoder channels); `out` receives the packed 16-bit operand:
  * [split][k-block][tap][n_cta][64 ch, 16-byte chunks XOR (row & 7)]. */

@@ -14,6 +14,27 @@ UNMODIFIED ``film_arch.Interpolator`` and the UNMODIFIED ``FILM_VFI.vfi`` (model
 unmodified Interpolator, saved to a temp file that the stubbed downloader returns) in the build container on
 ``synthetic_state_dict`` weights and stores their outputs in ``tests/golden/film_*.npz``;
 ``tests/test_oracle_film.py`` holds this file to them (max abs 1e-6) on every CPU run.
+
+16-bit-faithful mode.  ``interpolator_forward(..., operand="float16" | "bfloat16")`` (and its helpers) evaluate the same
+graph in float64 and round to 16 bits (``oracle.rife46.q16``) exactly where the CUDA library stores a 16-bit value, so
+that a comparison with the library measures accumulation order only.  With ``operand=None`` (the default) nothing is
+rounded and the fp32 graph above runs unchanged, bit for bit.  T is the operand type; where the library stores each
+tensor (csrc/film.cu, csrc/film_elem.cu, csrc/streamconv.cu: ``acc + shift``, the activation, then the T store):
+
+| tensor | library | operand mode |
+|---|---|---|
+| image pyramid | fp32 (``gather_rgb``, ``pool_rgb``) | float64, not rounded |
+| ``extract...convs.0.0`` (3 -> 64) | ``conv_rgb``: fp32 weights and bias, output stored in T | unrounded weights, ``round_T(lrelu(y))`` |
+| every other conv (streamconv) | weights packed to T, fp32 bias, fp32 accumulation, activation, T store | ``round_T(w)``, bias as is, ``round_T(act(y))`` |
+| pooled features, input of sub-level j >= 1 | ``pool16``: fp32 mean of four T values, stored in T | ``round_T(mean)`` |
+| up-sampled flow ``2 v`` | ``flow_up``, fp32 | float64 |
+| warped features inside the flow estimator | ``warp16``, stored in T | ``round_T(bilinear)`` |
+| flow estimator's 1x1 conv output (nf/2 channels) | T (streamconv) | ``round_T`` |
+| flow head (nf/2 -> 2) plus the up-sampled flow | ``flow_head``: T inputs, fp32 weights, fp32 output | unrounded weights, float64 |
+| aligned features (``warp16``, fscale 0.5) | T | ``round_T`` |
+| aligned images and the 0.5-scaled flows | ``misc64``, stored in T | ``round_T(warp(img))``, ``round_T(0.5 flow)`` |
+| fusion nearest resize | ``nearest16``, a copy | gather of T values |
+| output conv | ``out_rgb``: T inputs, fp32 weights, fp32 output, optional clamp | unrounded weights, float64 |
 """
 from __future__ import annotations
 
@@ -23,6 +44,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from oracle.rife46 import _dt, q16
 
 # Interpolator.__init__ defaults -- film_arch.py:377-386
 PYRAMID_LEVELS = 7
@@ -133,11 +156,17 @@ def synthetic_clip(n: int, h: int, w: int, seed: int = 1234) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------- model
-def _conv(sd, name: str, x: torch.Tensor, act: bool) -> torch.Tensor:
+def _conv(sd, name: str, x: torch.Tensor, act: bool, dt=None, packed: bool = True) -> torch.Tensor:
     """film_arch.py:784-798: Conv2d(padding='same') [+ LeakyReLU(0.2)].  For the even (2x2) kernels 'same' pads
-    0 rows/columns before and 1 after (ATen conv padding='same': total k-1, the extra one on the right/bottom)."""
+    0 rows/columns before and 1 after (ATen conv padding='same': total k-1, the extra one on the right/bottom).
+    With a 16-bit type ``dt``: float64, and for a ``packed`` (streamconv) layer the weight and the stored output rounded
+    to ``dt``; the CUDA-core layers (``packed=False``) keep fp32 weights and an fp32 output."""
     base = name + (".0" if act else "")
-    y = F.conv2d(x, sd[base + ".weight"], sd[base + ".bias"], padding="same")
+    if dt is None:
+        y = F.conv2d(x, sd[base + ".weight"], sd[base + ".bias"], padding="same")
+        return F.leaky_relu(y, LRELU_SLOPE) if act else y
+    w = sd[base + ".weight"]
+    y = F.conv2d(x, q16(w, dt).double() if packed else w.double(), sd[base + ".bias"].double(), padding="same")
     return F.leaky_relu(y, LRELU_SLOPE) if act else y
 
 
@@ -151,23 +180,25 @@ def build_image_pyramid(image: torch.Tensor, levels: int) -> List[torch.Tensor]:
     return pyr
 
 
-def sub_tree(sd, image: torch.Tensor, n: int) -> List[torch.Tensor]:
-    """SubTreeExtractor.forward, film_arch.py:102-121: all four conv pairs always run; pooling stops after n-1."""
+def sub_tree(sd, image: torch.Tensor, n: int, operand: Optional[str] = None) -> List[torch.Tensor]:
+    """SubTreeExtractor.forward, film_arch.py:102-121: all four conv pairs always run; pooling stops after n-1.
+    ``operand``: see the module docstring (every conv output and every pooled tensor is stored in T)."""
+    dt = _dt(operand)
     head = image
     pyr = []
     for i in range(SUB_LEVELS):
-        head = _conv(sd, f"extract.extract_sublevels.convs.{i}.0", head, True)
-        head = _conv(sd, f"extract.extract_sublevels.convs.{i}.1", head, True)
+        head = q16(_conv(sd, f"extract.extract_sublevels.convs.{i}.0", head, True, dt, packed=i > 0), dt)
+        head = q16(_conv(sd, f"extract.extract_sublevels.convs.{i}.1", head, True, dt), dt)
         pyr.append(head)
         if i < n - 1:
-            head = F.avg_pool2d(head, kernel_size=2, stride=2)
+            head = q16(F.avg_pool2d(head, kernel_size=2, stride=2), dt)
     return pyr
 
 
-def extract(sd, image_pyramid: List[torch.Tensor]) -> List[torch.Tensor]:
+def extract(sd, image_pyramid: List[torch.Tensor], operand: Optional[str] = None) -> List[torch.Tensor]:
     """FeatureExtractor.forward, film_arch.py:133-163 (cascaded feature pyramid)."""
     L = len(image_pyramid)
-    subs = [sub_tree(sd, image_pyramid[i], min(L - i, SUB_LEVELS)) for i in range(L)]
+    subs = [sub_tree(sd, image_pyramid[i], min(L - i, SUB_LEVELS), operand) for i in range(L)]
     out = []
     for i in range(L):
         f = subs[i][0]
@@ -186,40 +217,45 @@ def warp(image: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     H, W = fl.shape[2], fl.shape[3]
     ls1 = 1 - 1 / W
     ls2 = 1 - 1 / H
-    nf = fl.permute(0, 2, 3, 1) / torch.tensor([H * .5, W * .5], dtype=fl.dtype)[None, None, None]
+    nf = fl.permute(0, 2, 3, 1) / torch.tensor([H * .5, W * .5], dtype=fl.dtype, device=fl.device)[None, None, None]
     grid = torch.stack([
-        torch.linspace(-ls1, ls1, W, dtype=fl.dtype)[None, None, :] - nf[..., 1],
-        torch.linspace(-ls2, ls2, H, dtype=fl.dtype)[None, :, None] - nf[..., 0],
+        torch.linspace(-ls1, ls1, W, dtype=fl.dtype, device=fl.device)[None, None, :] - nf[..., 1],
+        torch.linspace(-ls2, ls2, H, dtype=fl.dtype, device=fl.device)[None, :, None] - nf[..., 0],
     ], dim=3)
     out = F.grid_sample(image, grid, mode="bilinear", padding_mode="border", align_corners=False)
     return out.reshape(image.shape)
 
 
-def flow_estimator(sd, prefix: str, num_convs: int, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """FlowEstimator.forward, film_arch.py:530-543."""
+def flow_estimator(sd, prefix: str, num_convs: int, a: torch.Tensor, b: torch.Tensor,
+                   operand: Optional[str] = None) -> torch.Tensor:
+    """FlowEstimator.forward, film_arch.py:530-543.  ``operand``: the 3x3 and 1x1 conv outputs stored in T, the head
+    (``flow_head``) with fp32 weights and an unrounded output."""
+    dt = _dt(operand)
     net = torch.cat([a, b], dim=1)
     for j in range(num_convs + 1):
-        net = _conv(sd, f"{prefix}._convs.{j}", net, True)
-    return _conv(sd, f"{prefix}._convs.{num_convs + 1}", net, False)
+        net = q16(_conv(sd, f"{prefix}._convs.{j}", net, True, dt), dt)
+    return _conv(sd, f"{prefix}._convs.{num_convs + 1}", net, False, dt, packed=False)
 
 
-def predict_flow(sd, pa: List[torch.Tensor], pb: List[torch.Tensor]) -> List[torch.Tensor]:
-    """PyramidFlowEstimator.forward, film_arch.py:567-616: residual flow pyramid, fine to coarse."""
+def predict_flow(sd, pa: List[torch.Tensor], pb: List[torch.Tensor], operand: Optional[str] = None) -> List[torch.Tensor]:
+    """PyramidFlowEstimator.forward, film_arch.py:567-616: residual flow pyramid, fine to coarse.  ``operand``: the warped
+    features are stored in T; the flows stay unrounded."""
+    dt = _dt(operand)
     levels = len(pa)
     n_spec = len(FLOW_CONVS) - 1  # len(self._predictors)
-    v = flow_estimator(sd, "predict_flow._predictor", FLOW_CONVS[3], pa[-1], pb[-1])
+    v = flow_estimator(sd, "predict_flow._predictor", FLOW_CONVS[3], pa[-1], pb[-1], operand)
     residuals = [v]
     for i in range(levels - 2, n_spec - 1, -1):
         v = F.interpolate(2 * v, size=pa[i].shape[2:4], mode="bilinear")
-        warped = warp(pb[i], v)
-        r = flow_estimator(sd, "predict_flow._predictor", FLOW_CONVS[3], pa[i], warped)
+        warped = q16(warp(pb[i], v), dt)
+        r = flow_estimator(sd, "predict_flow._predictor", FLOW_CONVS[3], pa[i], warped, operand)
         residuals.insert(0, r)
         v = r + v
     for k in range(n_spec):
         i = n_spec - 1 - k
         v = F.interpolate(2 * v, size=pa[i].shape[2:4], mode="bilinear")
-        warped = warp(pb[i], v)
-        r = flow_estimator(sd, f"predict_flow._predictors.{k}", FLOW_CONVS[i], pa[i], warped)
+        warped = q16(warp(pb[i], v), dt)
+        r = flow_estimator(sd, f"predict_flow._predictors.{k}", FLOW_CONVS[i], pa[i], warped, operand)
         residuals.insert(0, r)
         v = r + v
     return residuals
@@ -236,43 +272,52 @@ def flow_pyramid_synthesis(residuals: List[torch.Tensor]) -> List[torch.Tensor]:
     return pyr
 
 
-def fuse(sd, pyramid: List[torch.Tensor]) -> torch.Tensor:
-    """Fusion.forward, film_arch.py:258-296."""
+def fuse(sd, pyramid: List[torch.Tensor], operand: Optional[str] = None) -> torch.Tensor:
+    """Fusion.forward, film_arch.py:258-296.  ``operand``: every conv output but the output conv's stored in T (the
+    nearest resize copies T values)."""
+    dt = _dt(operand)
     net = pyramid[-1]
     n = SUB_LEVELS
     for k in range(n):
         i = n - 1 - k
         net = F.interpolate(net, size=pyramid[i].shape[2:4], mode="nearest")
-        net = _conv(sd, f"fuse.convs.{k}.0", net, False)
+        net = q16(_conv(sd, f"fuse.convs.{k}.0", net, False, dt), dt)
         net = torch.cat([pyramid[i], net], dim=1)
-        net = _conv(sd, f"fuse.convs.{k}.1", net, True)
-        net = _conv(sd, f"fuse.convs.{k}.2", net, True)
-    return _conv(sd, "fuse.output_conv", net, False)
+        net = q16(_conv(sd, f"fuse.convs.{k}.1", net, True, dt), dt)
+        net = q16(_conv(sd, f"fuse.convs.{k}.2", net, True, dt), dt)
+    return _conv(sd, "fuse.output_conv", net, False, dt, packed=False)
 
 
 def interpolator_forward(sd, x0: torch.Tensor, x1: torch.Tensor, batch_dt: torch.Tensor,
-                         debug: Optional[dict] = None) -> torch.Tensor:
+                         debug: Optional[dict] = None, operand: Optional[str] = None) -> torch.Tensor:
     """Interpolator.forward / debug_forward, film_arch.py:401-459.  x0, x1: [B,3,H,W] fp32, H and W multiples of
     64 are NOT required by the reference (the node feeds frames as they are); ``batch_dt`` only fixes the batch size:
-    the network always predicts the midpoint (:424-426)."""
+    the network always predicts the midpoint (:424-426).  ``operand``: see the module docstring; ``debug`` then also
+    receives ``forward_flow_levels`` / ``backward_flow_levels``, the flows of all seven levels."""
+    dt = _dt(operand)
     with torch.no_grad():
+        if dt is not None:
+            x0, x1 = x0.double(), x1.double()
         ip = [build_image_pyramid(x0, PYRAMID_LEVELS), build_image_pyramid(x1, PYRAMID_LEVELS)]
-        fp = [extract(sd, ip[0]), extract(sd, ip[1])]
-        fwd_res = predict_flow(sd, fp[0], fp[1])
-        bwd_res = predict_flow(sd, fp[1], fp[0])
-        fwd_pyr = flow_pyramid_synthesis(fwd_res)[:FUSION_PYRAMID_LEVELS]
-        bwd_pyr = flow_pyramid_synthesis(bwd_res)[:FUSION_PYRAMID_LEVELS]
+        fp = [extract(sd, ip[0], operand), extract(sd, ip[1], operand)]
+        fwd_res = predict_flow(sd, fp[0], fp[1], operand)
+        bwd_res = predict_flow(sd, fp[1], fp[0], operand)
+        fwd_all = flow_pyramid_synthesis(fwd_res)
+        bwd_all = flow_pyramid_synthesis(bwd_res)
+        fwd_pyr = fwd_all[:FUSION_PYRAMID_LEVELS]
+        bwd_pyr = bwd_all[:FUSION_PYRAMID_LEVELS]
         mid = torch.full_like(batch_dt, .5)
         bwd = [f * mid[:, 0] for f in bwd_pyr]          # multiply_pyramid, :727-742 (broadcast over the LAST axis
         fwd = [f * (1 - mid[:, 0]) for f in fwd_pyr]    # as written there; exact for batch 1 / equal scalars)
         to_warp = [[torch.cat([ip[k][l], fp[k][l]], dim=1) for l in range(FUSION_PYRAMID_LEVELS)] for k in (0, 1)]
-        fw = [warp(a, f) for a, f in zip(to_warp[0], bwd)]
-        bw = [warp(a, f) for a, f in zip(to_warp[1], fwd)]
-        aligned = [torch.cat([a, b, c, d], dim=1) for a, b, c, d in zip(fw, bw, bwd, fwd)]
+        fw = [q16(warp(a, f), dt) for a, f in zip(to_warp[0], bwd)]
+        bw = [q16(warp(a, f), dt) for a, f in zip(to_warp[1], fwd)]
+        aligned = [torch.cat([a, b, q16(c, dt), q16(d, dt)], dim=1) for a, b, c, d in zip(fw, bw, bwd, fwd)]
         if debug is not None:
             debug.update(feature_pyramids=fp, forward_residual=fwd_res, backward_residual=bwd_res,
-                         forward_flow=fwd_pyr, backward_flow=bwd_pyr, aligned=aligned)
-        return fuse(sd, aligned)
+                         forward_flow=fwd_pyr, backward_flow=bwd_pyr, aligned=aligned,
+                         forward_flow_levels=fwd_all, backward_flow_levels=bwd_all)
+        return fuse(sd, aligned, operand)
 
 
 # ------------------------------------------------------------------------------------------------- node

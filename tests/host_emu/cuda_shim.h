@@ -93,3 +93,4 @@ static inline cudaError_t emu_memset_async(void* d, int v, size_t n, cudaStream_
 #define cudaGetDevice(p) (*(p) = 0, cudaSuccess)
 #define cudaDeviceGetAttribute(v, a, d) (*(v) = 132, cudaSuccess)
 #define cudaStreamSynchronize(s) cudaSuccess
+#define cudaDeviceSynchronize() cudaSuccess

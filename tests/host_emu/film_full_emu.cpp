@@ -26,12 +26,28 @@ extern "C" const char* vfi_last_error(void) { return vfi::g_err.c_str(); }
 #include "../../comfyui-frame-interpolation_b200/csrc/film.cu"
 
 extern "C" {
+// a loaded context (operand_type: VFI_OPERAND_F16 / VFI_OPERAND_BF16) with every conv on the checker, for the C ABI's
+// forward and test hooks (vfi_film_forward, vfi_film_debug_state, vfi_film_debug_elem); NULL on failure
+vfi_ctx* emu_film_open(const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type) {
+  vfi_ctx* ctx = new vfi_ctx;
+  if (vfi_film_load(ctx, tensors, numel, n_tensors, operand_type) || vfi_film_debug_set_ref(ctx, 1)) {
+    vfi::film_destroy(ctx->film);
+    delete ctx;
+    return nullptr;
+  }
+  return ctx;
+}
+void emu_film_close(vfi_ctx* ctx) {
+  vfi::film_destroy(ctx->film);
+  delete ctx;
+}
+
 // flows (optional): the five finest levels of the forward, then of the backward flow pyramid, each [H_l, W_l, 2] fp32,
 // concatenated (what debug_forward returns as forward_flow_pyramid / backward_flow_pyramid, film_arch.py:417-419, :450-455)
 int emu_film(const float* const* tensors, const int64_t* numel, int n_tensors, const float* frames, int H, int W, int C,
-             int clamp01, float* out, float* flows) {
+             int clamp01, float* out, float* flows, int operand_type) {
   vfi_ctx ctx;
-  int rc = vfi_film_load(&ctx, tensors, numel, n_tensors, VFI_OPERAND_F16);
+  int rc = vfi_film_load(&ctx, tensors, numel, n_tensors, operand_type);
   if (rc) return rc;
   rc = vfi_film_debug_set_ref(&ctx, 1);
   if (rc) return rc;

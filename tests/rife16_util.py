@@ -126,11 +126,11 @@ def _worst(err: torch.Tensor, sel: torch.Tensor = None):
     return float(e.max()), tuple(reversed(idx))
 
 
-def compare(label: str, got, want, h: int, w: int, tol: Dict[str, float]):
-    """Max-abs comparison of (frame, flow, mask) over everything and over the border band; returns the report lines and
-    the list of failures (empty when every bound holds)."""
+def compare(label: str, got, want, h: int, w: int, tol: Dict[str, float], names=("frame", "flow", "mask")):
+    """Max-abs comparison of the planes ``names`` (default: frame, flow, mask) over everything and over the border band;
+    returns the report lines and the list of failures (empty when every bound holds)."""
     lines, fails = [], []
-    for name, g, r in zip(("frame", "flow", "mask"), got, want):
+    for name, g, r in zip(names, got, want):
         err = (g.to(r.device).double() - r.double()).abs()
         H, W = err.shape[1], err.shape[2]
         band = border_band(H, W, h, w, err.device)

@@ -50,7 +50,7 @@ def test_film_whole_path_on_host_matches_reference(emu, pkg, name):
     nflow = sum((h >> l) * (w >> l) * 2 for l in range(5))
     flows = torch.zeros(2 * nflow)
     rc = emu.emu_film(ptrs, numel, len(hold), C.c_void_p(fr.data_ptr()), h, w, 3, 0, C.c_void_p(out.data_ptr()),
-                      C.c_void_p(flows.data_ptr()))
+                      C.c_void_p(flows.data_ptr()), 0)
     assert rc >= 1000, (rc, emu.vfi_last_error())
     mse = float(((out.double() - ref.double()) ** 2).mean())
     psnr = 99.0 if mse == 0 else 10 * math.log10(1.0 / mse)
@@ -88,6 +88,7 @@ def test_film_two_pairs_in_one_call_on_host(emu, pkg):
     for i in (1,):   # the second pair is the one whose images sit at the non-trivial indices (1 and B + 1)
         one = torch.zeros(1, 64, 64, 3)
         pair = fr[i:i + 2].contiguous()
-        rc = emu.emu_film(ptrs, numel, len(hold), C.c_void_p(pair.data_ptr()), 64, 64, 4, 1, C.c_void_p(one.data_ptr()), None)
+        rc = emu.emu_film(ptrs, numel, len(hold), C.c_void_p(pair.data_ptr()), 64, 64, 4, 1, C.c_void_p(one.data_ptr()), None,
+                          0)
         assert rc >= 1000, emu.vfi_last_error()
         assert torch.equal(both[i], one[0]), i

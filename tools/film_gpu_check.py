@@ -9,7 +9,8 @@ Stages, each reported as one JSON line {"stage": ..., "ok": ..., ...}; exit code
                          on the CPU with the layer's real weights
   forward_ref / forward  Interpolator.forward through libvfi_b200.so with every conv on the CUDA-core checker / on the
                          wgmma kernel, vs the unmodified reference's output (tests/golden/film_net_*.npz): PSNR >= 50 dB
-                         and the five flow-pyramid levels within 0.05 px RMS
+                         on the frame only (the flows of every level, per pixel, and bf16 operands are checked by
+                         tests/test_gpu_zfilm16.py)
   node                   FILM_VFI.vfi vs the unmodified reference node's output (tests/golden/film_node_*.npz)
 The oracle / goldens are the checker here, never the thing measured.
 """
