@@ -15,6 +15,7 @@ SYMBOLS = [
     "vfi_film_load", "vfi_film_forward", "vfi_film_debug_set_ref", "vfi_film_debug_conv", "vfi_film_layer_plan",
     "vfi_film_last_macs", "vfi_film_debug_pack_host", "vfi_film_debug_state", "vfi_film_debug_elem",
     "vfi_sepconv_load", "vfi_sepconv_forward", "vfi_sepconv_debug_set_ref", "vfi_sepconv_debug_pack_host",
+    "vfi_sepconv_debug_state", "vfi_sepconv_debug_elem",
     "vfi_flavr_load", "vfi_flavr_forward", "vfi_flavr_debug_set_ref", "vfi_flavr_debug_conv", "vfi_flavr_layer_plan",
     "vfi_flavr_info",
     "vfi_ifrnet_load", "vfi_ifrnet_forward", "vfi_ifrnet_geometry", "vfi_ifrnet_debug_set_ref", "vfi_ifrnet_debug_conv",
@@ -83,6 +84,8 @@ def lib():
     L.vfi_sepconv_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]
     L.vfi_sepconv_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, vp, vp]
     L.vfi_sepconv_debug_set_ref.argtypes = [vp, i32]
+    L.vfi_sepconv_debug_state.argtypes = [vp, i32, i32, vp, i32, C.POINTER(i32)]
+    L.vfi_sepconv_debug_elem.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, f32, i32, vp]
     L.vfi_sepconv_debug_pack_host.argtypes = [i32, i32, i32, i32, i32, vp, vp, i64] + [C.POINTER(i32)] * 3
     L.vfi_flavr_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]
     L.vfi_flavr_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32, vp, vp]

@@ -63,7 +63,9 @@ struct SepState {
   StreamConvLayer hor[kRows][2];  // [row 1..4][3x3 + PReLU, 3x3 + skip]
   StreamConvLayer ver[kRows][2];  // [row 1..3][3x3 C_{r+1} -> C_r + PReLU, 3x3 added onto the row]
   StreamConvLayer head[4][2];     // Verone, Vertwo, Horone, Hortwo: [3x3 64 -> 64 + PReLU, 3x3 64 -> 51 (64 columns)]
-  SBuf x[kRows], S, T, U, V, K, coef[4], P1, P2, O1, O2, stats;
+  SBuf x[kRows], S, T, U, V, K, coef[4], P1, P2, O1, O2, stats, statp;
+  int last_B = 0;  // pairs and row sizes of the last forward (vfi_sepconv_debug_state)
+  int last_h[kRows] = {}, last_w[kRows] = {};
 };
 
 void sepconv_destroy(SepState* s) {
@@ -71,7 +73,7 @@ void sepconv_destroy(SepState* s) {
   for (void* p : s->allocs) cudaFree(p);
   for (int r = 0; r < kRows; ++r) s->x[r].release();
   for (SBuf* b : {&s->S, &s->T, &s->U, &s->V, &s->K, &s->coef[0], &s->coef[1], &s->coef[2], &s->coef[3], &s->P1, &s->P2, &s->O1,
-                  &s->O2, &s->stats})
+                  &s->O2, &s->stats, &s->statp})
     b->release();
   delete s;
 }
@@ -212,10 +214,14 @@ int forward(vfi_ctx* c, SepState* s, const float* frames, int n_frames, int H, i
   SCK(s->O1.ensure((size_t)B * 4 * px0 * 4));
   SCK(s->O2.ensure((size_t)B * 4 * px0 * 4));
   SCK(s->stats.ensure(2 * kMaxBatch * sizeof(double)));
+  SCK(s->statp.ensure((size_t)B * sep_stats_blocks(He, We) * 2 * sizeof(double)));
+  s->last_B = B;
+  std::copy(h, h + kRows, s->last_h);
+  std::copy(w, w + kRows, s->last_w);
   SRunner r{c, s, ctx_info(c).num_sms, st};
   const int op = s->op_type;
 
-  SRUN(r.ck(launch_sep_stats(frames, C, idx, B, H, W, He, We, (double*)s->stats.p, st), "sep_stats"));
+  SRUN(r.ck(launch_sep_stats(frames, C, idx, B, H, W, He, We, (double*)s->stats.p, (double*)s->statp.p, st), "sep_stats"));
   SRUN(r.ck(launch_sep_input_conv(op, frames, C, idx, B, H, W, He, We, (const double*)s->stats.p, s->in_w, s->in_b,
                                   s->enc_s0[1], s->S.p, st),
             "sep_input_conv"));
@@ -351,6 +357,99 @@ int vfi_sepconv_debug_set_ref(vfi_ctx* c, int use_ref) {
   SepState* s = c ? ctx_sep(c) : nullptr;
   if (!s) return sfail(VFI_E_STATE, "vfi_sepconv_load has not been called");
   s->use_ref = use_ref != 0;
+  return VFI_OK;
+}
+
+int vfi_sepconv_debug_state(vfi_ctx* c, int what, int index, void* out, int batch, int* shape) {
+  SepState* s = c ? ctx_sep(c) : nullptr;
+  if (!s || !s->loaded) return sfail(VFI_E_STATE, "vfi_sepconv_load has not been called");
+  if (!shape) return sfail(VFI_E_INVALID, "null argument");
+  if (!s->last_B) return sfail(VFI_E_STATE, "sepconv: no forward has run");
+  const int He = s->last_h[0], We = s->last_w[0];
+  size_t elem = 0;
+  const void* src = nullptr;
+  if (what == 0) {
+    if (index < 0 || index > 3) return sfail(VFI_E_INVALID, "sepconv: no such coefficient plane (0..3)");
+    const int sh[4] = {batch, kK, He, We};
+    std::copy(sh, sh + 4, shape);
+    elem = sizeof(float);
+    src = s->coef[index].p;
+  } else if (what == 1) {
+    if (index < 1 || index >= kRows) return sfail(VFI_E_INVALID, "sepconv: no such pyramid row (1..4)");
+    const int sh[4] = {batch, s->last_h[index], s->last_w[index], kC[index]};
+    std::copy(sh, sh + 4, shape);
+    elem = 2;
+    src = s->x[index].p;
+  } else if (what == 2) {
+    if (index != 0) return sfail(VFI_E_INVALID, "sepconv: the stats have no index");
+    const int sh[4] = {batch, 2, 1, 1};
+    std::copy(sh, sh + 4, shape);
+    elem = sizeof(double);
+    src = s->stats.p;
+  } else {
+    return sfail(VFI_E_INVALID, "sepconv: no such state (0 planes, 1 rows, 2 stats)");
+  }
+  if (!out) return VFI_OK;
+  if (batch < 1 || batch > s->last_B) return sfail(VFI_E_INVALID, "sepconv: batch larger than the last forward");
+  SCK(cudaSetDevice(ctx_info(c).device));
+  SCK(cudaDeviceSynchronize());
+  SCK(cudaMemcpy(out, src, (size_t)shape[0] * shape[1] * shape[2] * shape[3] * elem, cudaMemcpyDeviceToDevice));
+  SCK(cudaDeviceSynchronize());
+  return VFI_OK;
+}
+
+int vfi_sepconv_debug_elem(vfi_ctx* c, int kernel, const void* in0, const void* in1, const int32_t* f0, const int32_t* f1,
+                           int n_frames, void* out, int C, int B, int H, int W, int h, int w, float slope, int which,
+                           void* stream) {
+  SepState* s = c ? ctx_sep(c) : nullptr;
+  if (!s || !s->loaded) return sfail(VFI_E_STATE, "vfi_sepconv_load has not been called");
+  if (kernel < 0 || kernel > 8) return sfail(VFI_E_INVALID, "sepconv: no such element-wise kernel");
+  if (!in0 || !out || ((kernel == 1 || kernel == 8) && !in1)) return sfail(VFI_E_INVALID, "null argument");
+  if (B < 1 || B > kMaxBatch) return sfail(VFI_E_INVALID, "sepconv: B must be in [1,16]");
+  if (H < 1 || W < 1) return sfail(VFI_E_INVALID, "sepconv: empty launch");
+  const bool frames = kernel == 0 || kernel == 1 || kernel == 7;
+  SepPairIdx idx{};
+  if (frames) {
+    if (C < 3) return sfail(VFI_E_INVALID, "sepconv: frames need >= 3 channels");
+    if (!f0 || !f1) return sfail(VFI_E_INVALID, "null argument");
+    if (kernel == 7 && (which < 0 || which > 1)) return sfail(VFI_E_INVALID, "sepconv: pad_input pads frame 0 or 1");
+    for (int i = 0; i < B; ++i) {
+      if (f0[i] < 0 || f0[i] >= n_frames || f1[i] < 0 || f1[i] >= n_frames) return sfail(VFI_E_INVALID, "sepconv: frame index");
+      idx.f0[i] = f0[i];
+      idx.f1[i] = f1[i];
+    }
+  }
+  if (kernel >= 2 && kernel <= 5 && (C < 8 || (C & 7))) return sfail(VFI_E_INVALID, "sepconv: C must be a multiple of 8");
+  if ((kernel == 4 || kernel == 5) && (h < 1 || w < 1)) return sfail(VFI_E_INVALID, "sepconv: empty source");
+  if (kernel == 4 && (H > 2 * h || W > 2 * w)) return sfail(VFI_E_INVALID, "sepconv: up-sampling target larger than 2h x 2w");
+  if (kernel == 5 && (h < H || w < W)) return sfail(VFI_E_INVALID, "sepconv: crop source smaller than its target");
+  const int op = s->op_type;
+  const int He = H + (H & 1), We = W + (W & 1);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SCK(cudaSetDevice(ctx_info(c).device));
+  cudaError_t e = cudaSuccess;
+  switch (kernel) {
+    case 0:
+      SCK(s->statp.ensure((size_t)B * sep_stats_blocks(He, We) * 2 * sizeof(double)));
+      e = launch_sep_stats((const float*)in0, C, idx, B, H, W, He, We, (double*)out, (double*)s->statp.p, st);
+      break;
+    case 1:
+      e = launch_sep_input_conv(op, (const float*)in0, C, idx, B, H, W, He, We, (const double*)in1, s->in_w, s->in_b,
+                                s->enc_s0[1], out, st);
+      break;
+    case 2: e = launch_prelu_s2d16(op, in0, out, slope, C, B, H, W, st); break;
+    case 3: e = launch_prelu16(op, in0, out, slope, (size_t)B * H * W * C, st); break;
+    case 4: e = launch_prelu_up2_16(op, in0, out, slope, C, B, h, w, H, W, st); break;
+    case 5: e = launch_add_crop16(op, in0, h, w, out, C, B, H, W, st); break;
+    case 6: e = launch_sep_coeff_nchw(op, in0, 64, (float*)out, kK, B, H, W, st); break;
+    case 7:
+      e = launch_sep_pad_input((const float*)in0, C, idx, which, B, H, W, He + kK - 1, We + kK - 1, (float*)out, st);
+      break;
+    case 8: e = launch_sep_finish((const float*)in0, (const float*)in1, (float*)out, B, H, W, He, We, st); break;
+  }
+  ctx_add_launches(c, 1);
+  if (e == cudaErrorInvalidValue) return sfail(VFI_E_INVALID, "sepconv: launch refused");
+  if (e != cudaSuccess) return sfail(VFI_E_CUDA, std::string("sepconv: element-wise launch: ") + cudaGetErrorString(e));
   return VFI_OK;
 }
 

@@ -2,6 +2,7 @@
 // that is not a >= 64-channel conv or the separable-kernel op itself.  16-bit activations are dense NHWC tensors.
 //
 //   sep_stats       sum / sum of squares of the (replicate-padded-to-even) pair        :622-633 (mean, unbiased std)
+//                   per-block partials, then summed in a fixed order: the same call gives the same bits
 //   sep_input_conv  (x - mean) / (std + 1e-7) -> Conv2d(3,16,3,pad 1) per frame, cat -> PReLU -> space-to-depth
 //                   = the input of the first stride-2 conv                             :544-547, :640-642, :553
 //   prelu_s2d16     PReLU + space-to-depth (zero filled past an odd edge): input of a stride-2 conv   :110-131
@@ -46,9 +47,11 @@ inline int sgrid(size_t total, int threads) {
 
 __device__ __forceinline__ float prelu(float v, float s) { return v > 0.f ? v : s * v; }
 
-// ---- statistics of the padded pair: stats[2*b] = sum, stats[2*b+1] = sum of squares (double), over 2 frames x 3 x He x We
+// ---- statistics of the padded pair: stats[2*b] = sum, stats[2*b+1] = sum of squares (double), over 2 frames x 3 x He x We.
+// Block (x, b) writes its partial sums to partial[b][x]; sep_stats_sum_kernel adds them in index order (double atomics
+// across blocks would add them in whatever order the blocks finish, and the last bits would differ from call to call).
 __global__ void sep_stats_kernel(const float* __restrict__ frames, int cstride, SepPairIdx idx, int H, int W, int He, int We,
-                                 double* __restrict__ stats) {
+                                 double* __restrict__ partial) {
   const int b = blockIdx.y;
   const size_t per = (size_t)He * We;
   double s = 0.0, q = 0.0;
@@ -76,8 +79,34 @@ __global__ void sep_stats_kernel(const float* __restrict__ frames, int cstride, 
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    atomicAdd(stats + 2 * b, sh[0][0]);
-    atomicAdd(stats + 2 * b + 1, sh[1][0]);
+    double* p = partial + 2 * ((size_t)b * gridDim.x + blockIdx.x);
+    p[0] = sh[0][0];
+    p[1] = sh[1][0];
+  }
+}
+
+// one block per pair: stats[2*b], stats[2*b+1] = the sums of partial[b][0..nblk), in a fixed order
+__global__ void sep_stats_sum_kernel(const double* __restrict__ partial, int nblk, double* __restrict__ stats) {
+  const int b = blockIdx.x;
+  double s = 0.0, q = 0.0;
+  for (int i = threadIdx.x; i < nblk; i += blockDim.x) {
+    s += partial[2 * ((size_t)b * nblk + i)];
+    q += partial[2 * ((size_t)b * nblk + i) + 1];
+  }
+  __shared__ double sh[2][256];
+  sh[0][threadIdx.x] = s;
+  sh[1][threadIdx.x] = q;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) {
+      sh[0][threadIdx.x] += sh[0][threadIdx.x + o];
+      sh[1][threadIdx.x] += sh[1][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    stats[2 * b] = sh[0][0];
+    stats[2 * b + 1] = sh[1][0];
   }
 }
 
@@ -311,12 +340,13 @@ __global__ void sep_finish_kernel(const float* __restrict__ o1, const float* __r
 
 }  // namespace
 
+int sep_stats_blocks(int He, int We) { return sgrid((size_t)2 * He * We, 256 * 8); }
+
 cudaError_t launch_sep_stats(const float* frames, int cstride, const SepPairIdx& idx, int B, int H, int W, int He, int We,
-                             double* stats, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(stats, 0, (size_t)B * 2 * sizeof(double), st);
-  if (e != cudaSuccess) return e;
-  const dim3 g((unsigned)sgrid((size_t)2 * He * We, 256 * 8), (unsigned)B);
-  VFI_LAUNCH(sep_stats_kernel, g, 256, 0, st, frames, cstride, idx, H, W, He, We, stats);
+                             double* stats, double* partial, cudaStream_t st) {
+  const int nb = sep_stats_blocks(He, We);
+  VFI_LAUNCH(sep_stats_kernel, dim3((unsigned)nb, (unsigned)B), 256, 0, st, frames, cstride, idx, H, W, He, We, partial);
+  VFI_LAUNCH(sep_stats_sum_kernel, B, 256, 0, st, partial, nb, stats);
   return cudaGetLastError();
 }
 

@@ -244,8 +244,10 @@ struct SepPairIdx {  // source frames of every pair of a pass
 };
 struct SepState;
 void sepconv_destroy(SepState* s);  // sepconv.cu
+// stats [B, 2]; partial: scratch of B * sep_stats_blocks(He, We) * 2 doubles
+int sep_stats_blocks(int He, int We);
 cudaError_t launch_sep_stats(const float* frames, int cstride, const SepPairIdx& idx, int B, int H, int W, int He, int We,
-                             double* stats, cudaStream_t st);
+                             double* stats, double* partial, cudaStream_t st);
 cudaError_t launch_sep_input_conv(int op, const float* frames, int cstride, const SepPairIdx& idx, int B, int H, int W, int He,
                                   int We, const double* stats, const float* w, const float* bias, float slope, void* out,
                                   cudaStream_t st);

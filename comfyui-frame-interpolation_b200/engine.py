@@ -370,6 +370,7 @@ class SepconvEngine:
         ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
         numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
         check(self._L.vfi_sepconv_load(self._ctx, ptrs, numel, len(hold), OPERAND[dtype]))
+        self._dt16 = torch.bfloat16 if dtype == "bfloat16" else torch.float16
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -407,6 +408,29 @@ class SepconvEngine:
 
     def set_ref(self, use_ref: bool):
         check(self._L.vfi_sepconv_debug_set_ref(self._ctx, 1 if use_ref else 0))
+
+    def debug_state(self, what, index, batch):
+        """A tensor of the last forward as a CUDA tensor (vfi_sepconv_debug_state): what 0 = coefficient plane `index`
+        (0 Verone, 1 Vertwo, 2 Horone, 3 Hortwo) float32 [batch, 51, He, We]; 1 = pyramid row `index` (1..4) after
+        decoding, [batch, h, w, C] in the operand type; 2 = the per-pair (sum, sum of squares) float64 [batch, 2]."""
+        shape = (C.c_int * 4)()
+        check(self._L.vfi_sepconv_debug_state(self._ctx, what, index, None, batch, shape))
+        dt = {0: torch.float32, 1: self._dt16, 2: torch.float64}[what]
+        out = torch.empty(tuple(shape) if what != 2 else (batch, 2), dtype=dt, device=f"cuda:{self.device}")
+        check(self._L.vfi_sepconv_debug_state(self._ctx, what, index, out.data_ptr(), batch, shape))
+        return out
+
+    def debug_elem(self, kernel, in0, out, C_, B, H, W, in1=None, f0=None, f1=None, n_frames=0, h=0, w=0, slope=1.0,
+                   which=0):
+        """One sepconv_elem.cu kernel on CUDA tensors (vfi_sepconv_debug_elem; kernel ids in include/vfi_b200.h)."""
+        p = lambda t: None if t is None else t.data_ptr()   # noqa: E731
+        a = None if f0 is None else _i32(f0)
+        b = None if f1 is None else _i32(f1)
+        st = torch.cuda.current_stream(in0.device).cuda_stream
+        check(self._L.vfi_sepconv_debug_elem(self._ctx, kernel, p(in0), p(in1), None if a is None else a.ctypes.data,
+                                             None if b is None else b.ctypes.data, int(n_frames), p(out), int(C_), B, H, W,
+                                             h, w, float(slope), int(which), st))
+        return out
 
     def launch_count(self) -> int:
         return int(self._L.vfi_launch_count(self._ctx))

@@ -195,6 +195,27 @@ int vfi_sepconv_forward(vfi_ctx* ctx, const float* frames, int n_frames, int H, 
  * vfi_sepconv_load (a 3x3 conv packed as a stride-1 layer, or as the 2x2 conv over the space-to-depth input that runs
  * its stride-2 form). */
 int vfi_sepconv_debug_set_ref(vfi_ctx* ctx, int use_ref);
+/* Test hooks.  vfi_sepconv_debug_state copies a tensor of the last forward into a caller DEVICE buffer and synchronises;
+ * `shape` (4 ints) receives its shape; `out` NULL only returns the shape.
+ *   what 0: coefficient plane `index` (0 Verone, 1 Vertwo, 2 Horone, 3 Hortwo), [batch, 51, He, We] float32
+ *   what 1: pyramid row `index` (1..4) after decoding, [batch, h_r, w_r, C_r] 16-bit
+ *   what 2: per-pair statistics (sum, sum of squares of the padded pair), [batch, 2] double; index 0
+ * vfi_sepconv_debug_elem runs one kernel of sepconv_elem.cu on caller DEVICE tensors with the loaded operand type;
+ * asynchronous on `stream`.  He = H + (H & 1), We = W + (W & 1); 16-bit tensors are packed NHWC.  kernel:
+ *   0 stats         in0 frames [n_frames, H, W, C] float32, pairs (f0[i], f1[i]) (HOST) -> out [B, 2] double
+ *   1 input_conv    in0 frames, in1 stats [B, 2] double -> out [B, He/2, We/2, 128] (netInput + PReLU, space-to-depth)
+ *   2 prelu_s2d16   in0 [B, H, W, C] -> out [B, ceil(H/2), ceil(W/2), 4 C], PReLU `slope`
+ *   3 prelu16       in0 [B, H, W, C] -> out [B, H, W, C], PReLU `slope`
+ *   4 prelu_up2_16  in0 [B, h, w, C] -> out [B, H, W, C] (H <= 2h, W <= 2w), PReLU `slope` then bilinear x2
+ *   5 add_crop16    out [B, H, W, C] += in0 [B, h, w, C][:, :H, :W] (h >= H, w >= W)
+ *   6 coeff_nchw    in0 [B, H, W, 64] -> out [B, 51, H, W] float32
+ *   7 pad_input     in0 frames, frame f0[i] (which 0) or f1[i] (which 1) -> out [B, 4, He + 50, We + 50] float32
+ *   8 finish        in0 / in1 [B, 4, He, We] float32 -> out [B, H, W, 3] float32
+ * Arguments are checked before anything runs; a refused call returns VFI_E_INVALID, names the reason and writes nothing. */
+int vfi_sepconv_debug_state(vfi_ctx* ctx, int what, int index, void* out, int batch, int* shape);
+int vfi_sepconv_debug_elem(vfi_ctx* ctx, int kernel, const void* in0, const void* in1, const int32_t* f0, const int32_t* f1,
+                           int n_frames, void* out, int C, int B, int H, int W, int h, int w, float slope, int which,
+                           void* stream);
 int vfi_sepconv_debug_pack_host(int stride2, int cin, int cout, int n_total, int operand_type, const float* w, uint16_t* out,
                                 int64_t out_cap, int* c0, int* n_cta, int* nsplit);
 

@@ -13,8 +13,9 @@ static SepPairIdx pair01() {
 
 extern "C" {
 void emu_stats(const float* frames, int cstride, int H, int W, int He, int We, double* stats) {
-  stats[0] = stats[1] = 0.0;
-  sep_stats_kernel(frames, cstride, pair01(), H, W, He, We, stats);
+  double partial[2] = {0.0, 0.0};
+  sep_stats_kernel(frames, cstride, pair01(), H, W, He, We, partial);
+  sep_stats_sum_kernel(partial, 1, stats);
 }
 void emu_input_conv(const float* frames, int cstride, int H, int W, int He, int We, const double* stats, const float* w,
                     const float* bias, float slope, uint16_t* out) {

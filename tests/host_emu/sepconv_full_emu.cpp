@@ -28,6 +28,26 @@ extern "C" const char* vfi_last_error(void) { return vfi::g_err.c_str(); }
 #include "../../comfyui-frame-interpolation_b200/csrc/sepconv.cu"
 
 extern "C" {
+// a loaded context (operand_type: VFI_OPERAND_F16 / VFI_OPERAND_BF16) with every conv on the checker, for the C ABI's
+// forward and test hooks (vfi_sepconv_forward, vfi_sepconv_debug_state, vfi_sepconv_debug_elem); NULL on failure
+vfi_ctx* emu_sepconv_open(const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type) {
+  vfi_ctx* ctx = new vfi_ctx;
+  if (vfi_sepconv_load(ctx, tensors, numel, n_tensors, operand_type) || vfi_sepconv_debug_set_ref(ctx, 1)) {
+    vfi::sepconv_destroy(ctx->sep);
+    delete ctx;
+    return nullptr;
+  }
+  return ctx;
+}
+void emu_sepconv_close(vfi_ctx* ctx) {
+  vfi::sepconv_destroy(ctx->sep);
+  delete ctx;
+}
+// the separable-convolution op (csrc/ops.cu, the launcher behind vfi_sepconv and the forward's two op launches)
+int emu_sepconv_op(const float* in, const float* ver, const float* hor, float* out, int N, int C, int H, int W, int Kv, int Kh) {
+  return (int)vfi::launch_sepconv(in, ver, hor, out, N, C, H, W, Kv, Kh, nullptr);
+}
+
 // weights in, one pair in, one frame out - everything through the product's own vfi_sepconv_load / vfi_sepconv_forward
 // coef (optional): [4][51][He][We] fp32 = the coefficient planes of the heads Verone, Vertwo, Horone, Hortwo
 int emu_sepconv(const float* const* tensors, const int64_t* numel, int n_tensors, const float* frames, int H, int W, int C,
