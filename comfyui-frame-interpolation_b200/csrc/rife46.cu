@@ -189,7 +189,9 @@ struct vfi_ctx {
   TapConvLayer head[3];          // arch 4.17 / 4.26: Head cnn1, cnn2 (+ LeakyReLU), cnn3 (ConvTranspose), 32 (padded) channels
   DevBuf hA, hB;                 // arch 4.17: half-resolution 32-channel scratch of the head (ping-pong)
   int ws_Hp = 0, ws_Wp = 0, ws_B = 0;
-  FlowState last_fs{};
+  FlowState last_fs{};  // the last pass: its levels, flow / mask planes and which levels those hold (debug_state)
+  float4* last_F = nullptr;
+  float* last_M = nullptr;
   int last_lo = 0;
   bool last_have_base = false;
   DevBuf dbgF, dbgM;
@@ -338,6 +340,10 @@ struct Geometry {
   int nb;  // blocks: 4, arch 4.26: 5
   int s[kMaxBlocks];  // block scale (>= 1); 1 for an up-scaled block
   int k[kMaxBlocks];  // 1, or the up-scaling factor 2 / 4 of a block whose scale is 1/k (node scale_factor 2 / 4)
+  // first block whose front visits every full-resolution pixel (scale <= 2, or up-scaled); the blocks before it are the
+  // "coarse" blocks, which run over a whole coarse span of pairs (forward_span)
+  int dense;
+  size_t level_px(int i) const { return (size_t)(Hp * k[i] / s[i]) * (Wp * k[i] / s[i]); }  // block i's grid, per pair
 };
 
 int make_geometry(int arch, int H, int W, float scale_factor, Geometry* g) {
@@ -364,19 +370,85 @@ int make_geometry(int arch, int H, int W, float scale_factor, Geometry* g) {
                   "padded size / scale is not a multiple of 4: the reference fails with a shape mismatch for this "
                   "size and scale_factor as well");
   }
+  g->dense = g->nb;
+  for (int i = g->nb - 1; i >= 1; --i)
+    if (g->s[i] <= 2) g->dense = i;
   return VFI_OK;
 }
 
-int ensure_workspace(vfi_ctx* c, const Geometry& g, int B, int n_frames_window) {
+// Workspace bytes of block i per pair: its s2d block input (x), conv0.0 output (c00), one ResConv feature map (featA / featB
+// each) and its output level (tF, tM and arch 4.26's tE).
+struct BlockBytes { size_t x, c00, feat, level; };
+
+BlockBytes block_bytes(const vfi_ctx* c, const Geometry& g, int i) {
+  const size_t px = g.level_px(i);
+  return {px / 4 * (c->arch != 46 ? 128 : 64) * 2, px / 16 * 2 * kBlockC[i] * 2, px / 16 * kBlockC[i] * 2,
+          px * (sizeof(float4) + sizeof(float) + (block_has_layer(c->arch, i, LAYER_LASTFEAT) ? 16 : 0))};
+}
+
+// Byte budgets of the wide spans (workspace at the blocks' own sizes: the shared x / c00 / featA / featB plus the output
+// levels, and for the first dense block the full-resolution flow / mask planes it stores).  At 1080p the coarse blocks of
+// 4.6 cost 15.8 MB per pair, so 1 GiB holds one span of a whole 63-pair forward call; the first dense block (block 2 of
+// 4.6, scale 2) costs 169 MB per pair, so 4 GiB holds spans of 24 pairs (DESIGN.md section 4.3 has the measured widths).
+// A build may set other budgets (the host-emulation tests use a few hundred kB, so that tiny frames take several spans).
+#ifndef VFI_COARSE_BUDGET_BYTES
+#define VFI_COARSE_BUDGET_BYTES (1ull << 30)
+#endif
+#ifndef VFI_MID_BUDGET_BYTES
+#define VFI_MID_BUDGET_BYTES (4ull << 30)
+#endif
+constexpr size_t kCoarseBudget = VFI_COARSE_BUDGET_BYTES;
+constexpr size_t kMidBudget = VFI_MID_BUDGET_BYTES;
+
+// How many pairs each block runs over per launch.  The coarse blocks [0, g.dense) run over coarse spans of Bc pairs; the
+// first dense block, when another block follows it, over middle spans of Bm pairs inside them; the other blocks and
+// `final` over passes of B = `batch` pairs inside those (a middle span ends early where its coarse span ends).  Bc and Bm
+// are whole numbers of B, so the passes fall where they would if every block ran pass by pass.
+struct Widths {
+  int Bc, Bm, B;
+  int dense;  // g.dense
+  int mid;    // g.dense when that block runs over middle spans, else -1 (it is the last block, or up-scaled; Bm = B)
+  int of(int i) const { return i < dense ? Bc : i == mid ? Bm : B; }
+};
+
+// The most pairs whose bytes per pair fit `budget`, as a whole number of `unit`, at least `unit` and at most n_tasks
+int fit_width(size_t per_pair, size_t budget, int unit, int n_tasks) {
+  const int fit = (int)std::min<size_t>(budget / per_pair, 1 << 20);
+  return std::min(n_tasks, std::max(unit, fit / unit * unit));
+}
+
+Widths span_widths(const vfi_ctx* c, const Geometry& g, int B, int n_tasks) {
+  Widths w{B, B, B, g.dense, -1};
+  if (g.dense + 1 < g.nb && g.k[g.dense] == 1) {
+    const BlockBytes b = block_bytes(c, g, g.dense);
+    const size_t per_pair = b.x + b.c00 + 2 * b.feat + b.level + (size_t)g.Hp * g.Wp * (sizeof(float4) + sizeof(float));
+    w.mid = g.dense;
+    w.Bm = fit_width(per_pair, kMidBudget, B, n_tasks);
+  }
+  size_t x = 0, c00 = 0, feat = 0, level = 0;
+  for (int i = 0; i < g.dense; ++i) {
+    const BlockBytes b = block_bytes(c, g, i);
+    x = std::max(x, b.x);
+    c00 = std::max(c00, b.c00);
+    feat = std::max(feat, b.feat);
+    level += b.level;
+  }
+  w.Bc = fit_width(x + c00 + 2 * feat + level, kCoarseBudget, B, n_tasks);
+  return w;
+}
+
+int ensure_workspace(vfi_ctx* c, const Geometry& g, const Widths& w, int n_frames_window) {
   size_t x = 0, c00 = 0, feat = 0;
   for (int i = 0; i < g.nb; ++i) {
-    const size_t Hs = (size_t)g.Hp * g.k[i] / g.s[i], Ws = (size_t)g.Wp * g.k[i] / g.s[i];
-    x = std::max(x, (size_t)B * (Hs / 2) * (Ws / 2) * (c->arch != 46 ? 128 : 64) * 2);
-    c00 = std::max(c00, (size_t)B * (Hs / 4) * (Ws / 4) * 2 * kBlockC[i] * 2);
-    feat = std::max(feat, (size_t)B * (Hs / 4) * (Ws / 4) * kBlockC[i] * 2);
-    CK(c->tF[i].ensure((size_t)B * Hs * Ws * sizeof(float4)));  // block output T_i (flow increments at 1/s_i)
-    CK(c->tM[i].ensure((size_t)B * Hs * Ws * sizeof(float)));
-    if (block_has_layer(c->arch, i, LAYER_LASTFEAT)) CK(c->tE[i].ensure((size_t)B * Hs * Ws * 16));
+    const size_t n = w.of(i);
+    const BlockBytes b = block_bytes(c, g, i);
+    const size_t px = n * g.level_px(i);
+    x = std::max(x, n * b.x);
+    c00 = std::max(c00, n * b.c00);
+    feat = std::max(feat, n * b.feat);
+    CK(c->tF[i].ensure(px * sizeof(float4)));  // block output T_i (flow increments at 1/s_i)
+    CK(c->tM[i].ensure(px * sizeof(float)));
+    if (block_has_layer(c->arch, i, LAYER_LASTFEAT)) CK(c->tE[i].ensure(px * 16));
   }
   const size_t px = (size_t)g.Hp * g.Wp;
   CK(c->imgs.ensure((size_t)n_frames_window * px * sizeof(float4)));
@@ -391,8 +463,8 @@ int ensure_workspace(vfi_ctx* c, const Geometry& g, int B, int n_frames_window) 
     CK(c->hA.ensure((size_t)(kMaxBatch + 2) * (px / 4) * 32 * 2));
     CK(c->hB.ensure((size_t)(kMaxBatch + 2) * (px / 4) * 32 * 2));
   }
-  CK(c->flow.ensure((size_t)B * px * sizeof(float4)));
-  CK(c->mask.ensure((size_t)B * px * sizeof(float)));
+  CK(c->flow.ensure((size_t)std::max(w.Bm, w.B) * px * sizeof(float4)));  // written by the first dense block onwards
+  CK(c->mask.ensure((size_t)std::max(w.Bm, w.B) * px * sizeof(float)));
   CK(c->x.ensure(x));
   CK(c->c00.ensure(c00));
   CK(c->featA.ensure(feat));
@@ -433,105 +505,185 @@ int run_encode(vfi_ctx* c, const Geometry& g, int f, int n, cudaStream_t st) {
   return VFI_OK;
 }
 
-// one internal pass: tasks (indices into the prepared frame window c->imgs) -> out [n, H, W, 3]
-int forward_pass(vfi_ctx* c, const Geometry& g, const BatchTasks& tasks, int H, int W, float* out, cudaStream_t st) {
-  const int B = tasks.n;
+// group ids of vfi_rife_profile: 10 * block + {0 front, 1 conv0.0, 2 conv0.1, 3 the 8 ResConvs, 4 lastconv(s)}, 90 final.
+// A coarse block's spans cover its whole coarse span of pairs, a dense block's one pass.
+void span_begin(vfi_ctx* c, int id, cudaStream_t st) {
+  if (!c->profile) return;
+  vfi_ctx::ProfSpan sp{id, nullptr, nullptr};
+  cudaEventCreate(&sp.e0);
+  cudaEventCreate(&sp.e1);
+  cudaEventRecord(sp.e0, st);
+  c->prof_spans.push_back(sp);
+}
+
+void span_end(vfi_ctx* c, cudaStream_t st) {
+  if (c->profile) cudaEventRecord(c->prof_spans.back().e1, st);
+}
+
+// The tasks of a forward span: frame indices into the prepared frame window c->imgs, and timesteps
+struct SpanTasks {
+  const int32_t* f0;
+  const int32_t* f1;
+  const float* t;
+  BatchTasks batch(int pos, int n) const {  // n <= kMaxBatch
+    BatchTasks bt{};
+    bt.n = n;
+    for (int i = 0; i < n; ++i) {
+      bt.f0[i] = f0[pos + i];
+      bt.f1[i] = f1[pos + i];
+      bt.t[i] = t[pos + i];
+    }
+    return bt;
+  }
+};
+
+// The block output levels (4.26: and feature levels) and the full-resolution flow / mask planes, seen from one pair
+struct Levels {
+  FlowState fs;
+  uint8_t* e[kMaxBlocks];  // arch 4.26: tE
+  float4* F;               // accumulated full-resolution flow / mask, written only by "dense" fronts
+  float* M;
+};
+
+// lv with levels [0, upto) advanced by p pairs, and with `planes` the flow / mask planes too
+Levels advance(Levels lv, const Geometry& g, int upto, bool planes, int p) {
+  for (int j = 0; j < upto; ++j) {
+    lv.fs.f[j] += (size_t)p * g.level_px(j);
+    lv.fs.m[j] += (size_t)p * g.level_px(j);
+    if (lv.e[j]) lv.e[j] += (size_t)p * g.level_px(j) * 16;
+  }
+  if (planes) {
+    lv.F += (size_t)p * g.Hp * g.Wp;
+    lv.M += (size_t)p * g.Hp * g.Wp;
+  }
+  return lv;
+}
+
+// Block i over the n pairs tk[pos, pos + n): its front, then conv0.0, conv0.1, the 8 ResConvs and lastconv (4.26: and the
+// feature conv), each one tap-conv launch over all n pairs.  lv: the earlier levels and the flow / mask planes at pair `pos`;
+// block i's own level is written from its first pair.  lo / have_base: which levels the flow / mask planes hold, read and
+// advanced by dense and up-scaled fronts.  A front runs in chunks of at most kMaxBatch tasks (BatchTasks); a chunk at pair
+// `at` writes the block input and reads and writes the earlier levels and the planes there.
+int run_block(vfi_ctx* c, const Geometry& g, int i, const SpanTasks& tk, int pos, int n, const Levels& lv, int& lo,
+              bool& have_base, cudaStream_t st) {
   const float4* imgs = (const float4*)c->imgs.p;
   const uint2* imgs_h = (const uint2*)c->imgs_h.p;
   const void* feats = c->arch != 46 ? c->feats.p : nullptr;
-  const int nb = g.nb;
-  float4* F = (float4*)c->flow.p;  // accumulated full-resolution flow / mask, written only by "dense" fronts
-  float* M = (float*)c->mask.p;
-  FlowState fs{};
-  fs.n = nb;
-  for (int i = 0; i < nb; ++i) {
-    fs.f[i] = (float4*)c->tF[i].p;
-    fs.m[i] = (float*)c->tM[i].p;
-    fs.s[i] = g.s[i];
-  }
-  fs.mask_replace = (c->arch != 46) ? 1 : 0;
-  int dense = nb;  // first block whose front visits every full-resolution pixel (scale <= 2)
-  for (int i = nb - 1; i >= 1; --i)
-    if (g.s[i] <= 2) dense = i;
-  bool have_base = false;
-  int lo = 0;  // levels [lo, i) are not yet folded into F
-  // group ids of vfi_rife_profile: 10 * block + {0 front, 1 conv0.0, 2 conv0.1, 3 the 8 ResConvs, 4 lastconv(s)}, 90 final
-  auto span_begin = [&](int id) {
-    if (!c->profile) return;
-    vfi_ctx::ProfSpan sp{id, nullptr, nullptr};
-    cudaEventCreate(&sp.e0);
-    cudaEventCreate(&sp.e1);
-    cudaEventRecord(sp.e0, st);
-    c->prof_spans.push_back(sp);
-  };
-  auto span_end = [&]() {
-    if (c->profile) cudaEventRecord(c->prof_spans.back().e1, st);
-  };
-  for (int i = 0; i < nb; ++i) {
-    const int s = g.s[i];
-    const int Hs = g.Hp * g.k[i] / s, Ws = g.Wp * g.k[i] / s;
-    const void* pfeat = (c->arch == 426 && i > 0) ? c->tE[i - 1].p : nullptr;  // previous block's 8 feature channels
-    const int ps = i > 0 ? g.s[i - 1] : 1;
-    span_begin(10 * i);
-    if (g.k[i] > 1) {
-      // up-scaled block: fold every level so far into the dense planes, build the k-times finer input from them
-      if (i == 0) return fail(VFI_E_INVALID, "the first block cannot be up-scaled");
-      if (lo < i) {
-        FlowState part = fs;
-        part.n = i;
-        LAUNCH(launch_materialize(part, lo, have_base ? F : nullptr, have_base ? M : nullptr, F, M, B, g.Hp, g.Wp, st));
-        have_base = true;
-        lo = i;
-      }
-      LAUNCH(launch_front_up(c->op_type, c->arch, imgs_h, feats, pfeat, ps, g.k[i - 1], F, M, tasks, g.Hp, g.Wp, g.k[i], c->x.p,
-                             st));
-    } else if (i == 0 || i < dense) {
-      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, pfeat, ps, fs, i, 0, nullptr, nullptr, nullptr, nullptr,
-                          tasks, g.Hp, g.Wp, s, c->x.p, st));
-    } else {
-      // a dense front stores the accumulated flow, the last one too: `final` adding two levels per pixel is instruction bound
-      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, pfeat, ps, fs, i, lo, have_base ? F : nullptr,
-                          have_base ? M : nullptr, F, M, tasks, g.Hp, g.Wp, s, c->x.p, st));
+  const FlowState& fs = lv.fs;
+  const int s = g.s[i];
+  const int Hs = g.Hp * g.k[i] / s, Ws = g.Wp * g.k[i] / s;
+  const int ps = i > 0 ? g.s[i - 1] : 1;
+  const bool dense = i >= g.dense;
+  span_begin(c, 10 * i, st);
+  if (g.k[i] > 1) {
+    // up-scaled block: fold every level so far into the dense planes, build the k-times finer input from them
+    if (i == 0) return fail(VFI_E_INVALID, "the first block cannot be up-scaled");
+    if (n > kMaxBatch) return fail(VFI_E_STATE, "an up-scaled block runs at most 16 pairs at once");
+    if (lo < i) {
+      FlowState part = fs;
+      part.n = i;
+      LAUNCH(launch_materialize(part, lo, have_base ? lv.F : nullptr, have_base ? lv.M : nullptr, lv.F, lv.M, n, g.Hp, g.Wp,
+                                st));
       have_base = true;
       lo = i;
     }
-    span_end();
-    span_begin(10 * i + 1);
-    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV00], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, B, Hs / 2, Ws / 2,
-                          c->num_sms, TAPCONV_PLANNED, st));
-    span_end();
-    span_begin(10 * i + 2);
-    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV01], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, B, Hs / 4, Ws / 4,
-                          c->num_sms, TAPCONV_PLANNED, st));
-    span_end();
-    void* a = c->featA.p;
-    void* b = c->featB.p;
-    span_begin(10 * i + 3);
-    for (int j = 0; j < 8; ++j) {
-      LAUNCH(launch_tapconv(c->layers[i][LAYER_RESCONV + j], c->op_type, a, b, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
-                            TAPCONV_PLANNED, st));
-      std::swap(a, b);
+    LAUNCH(launch_front_up(c->op_type, c->arch, imgs_h, feats, i > 0 ? lv.e[i - 1] : nullptr, ps, g.k[i - 1], lv.F, lv.M,
+                           tk.batch(pos, n), g.Hp, g.Wp, g.k[i], c->x.p, st));
+  } else {
+    // a dense front stores the accumulated flow, the last one too: `final` adding two levels per pixel is instruction bound
+    const size_t x_pair = block_bytes(c, g, i).x;
+    for (int at = 0; at < n; at += kMaxBatch) {
+      const Levels ck = advance(lv, g, i, true, at);
+      LAUNCH(launch_front(c->op_type, c->arch, imgs, imgs_h, feats, i > 0 ? ck.e[i - 1] : nullptr, ps, ck.fs, i,
+                          dense ? lo : 0, dense && have_base ? ck.F : nullptr, dense && have_base ? ck.M : nullptr,
+                          dense ? ck.F : nullptr, dense ? ck.M : nullptr, tk.batch(pos + at, std::min(kMaxBatch, n - at)),
+                          g.Hp, g.Wp, s, (uint8_t*)c->x.p + at * x_pair, st));
     }
-    span_end();
-    span_begin(10 * i + 4);
-    LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTCONV], c->op_type, a, nullptr, fs.f[i], fs.m[i], B, Hs / 4, Ws / 4, c->num_sms,
-                          TAPCONV_PLANNED, st));
-    if (block_has_layer(c->arch, i, LAYER_LASTFEAT))  // the 8 feature channels of lastconv, for the next block's input
-      LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTFEAT], c->op_type, a, c->tE[i].p, nullptr, nullptr, B, Hs / 4, Ws / 4, c->num_sms,
-                            TAPCONV_PLANNED, st));
-    if (g.k[i] > 1) {  // the up-scaled block's output goes straight back onto the dense planes
-      LAUNCH(launch_fold_down(fs.f[i], fs.m[i], g.k[i], F, M, B, g.Hp, g.Wp, fs.mask_replace, st));
-      lo = i + 1;
+    if (dense) {
+      have_base = true;
+      lo = i;
     }
-    span_end();
   }
-  span_begin(90);
-  LAUNCH(launch_final(imgs, fs, lo, have_base ? F : nullptr, have_base ? M : nullptr, tasks, g.Hp, g.Wp, H, W, out, st));
-  span_end();
-  c->last_fs = fs;
-  c->last_lo = lo;
-  c->last_have_base = have_base;
-  c->ws_B = B;
+  span_end(c, st);
+  span_begin(c, 10 * i + 1, st);
+  LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV00], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, n, Hs / 2, Ws / 2,
+                        c->num_sms, TAPCONV_PLANNED, st));
+  span_end(c, st);
+  span_begin(c, 10 * i + 2, st);
+  LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV01], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, n, Hs / 4, Ws / 4,
+                        c->num_sms, TAPCONV_PLANNED, st));
+  span_end(c, st);
+  void* a = c->featA.p;
+  void* b = c->featB.p;
+  span_begin(c, 10 * i + 3, st);
+  for (int j = 0; j < 8; ++j) {
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_RESCONV + j], c->op_type, a, b, nullptr, nullptr, n, Hs / 4, Ws / 4, c->num_sms,
+                          TAPCONV_PLANNED, st));
+    std::swap(a, b);
+  }
+  span_end(c, st);
+  span_begin(c, 10 * i + 4, st);
+  LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTCONV], c->op_type, a, nullptr, fs.f[i], fs.m[i], n, Hs / 4, Ws / 4, c->num_sms,
+                        TAPCONV_PLANNED, st));
+  if (block_has_layer(c->arch, i, LAYER_LASTFEAT))  // the 8 feature channels of lastconv, for the next block's input
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_LASTFEAT], c->op_type, a, lv.e[i], nullptr, nullptr, n, Hs / 4, Ws / 4,
+                          c->num_sms, TAPCONV_PLANNED, st));
+  if (g.k[i] > 1) {  // the up-scaled block's output goes straight back onto the dense planes
+    LAUNCH(launch_fold_down(fs.f[i], fs.m[i], g.k[i], lv.F, lv.M, n, g.Hp, g.Wp, fs.mask_replace, st));
+    lo = i + 1;
+  }
+  span_end(c, st);
+  return VFI_OK;
+}
+
+// One coarse span: tasks tk[0, n) -> out [n, H, W, 3], n <= w.Bc.  The coarse blocks (before g.dense) run over all n pairs
+// at once, so that their small grids fill the GPU; the first dense block over middle spans of w.Bm pairs; the other blocks
+// and `final` in passes of w.B pairs.  Per-pair arithmetic does not depend on how many pairs a launch covers, so the frames
+// are the same for any widths.  The workspace holds each block's width of pairs (ensure_workspace).
+int forward_span(vfi_ctx* c, const Geometry& g, const SpanTasks& tk, int n, const Widths& w, int H, int W, float* out,
+                 cudaStream_t st) {
+  Levels lv{};
+  lv.fs.n = g.nb;
+  for (int i = 0; i < g.nb; ++i) {
+    lv.fs.f[i] = (float4*)c->tF[i].p;
+    lv.fs.m[i] = (float*)c->tM[i].p;
+    lv.fs.s[i] = g.s[i];
+    lv.e[i] = (uint8_t*)c->tE[i].p;
+  }
+  lv.fs.mask_replace = (c->arch != 46) ? 1 : 0;
+  lv.F = (float4*)c->flow.p;
+  lv.M = (float*)c->mask.p;
+  int r, lo = 0;  // levels [lo, i) are not yet folded into the dense planes
+  bool have_base = false;
+  for (int i = 0; i < g.dense; ++i)
+    if ((r = run_block(c, g, i, tk, 0, n, lv, lo, have_base, st))) return r;
+  const int mid_end = w.mid >= 0 ? w.mid + 1 : g.dense;
+  for (int mpos = 0; mpos < n; mpos += w.Bm) {
+    const int mn = std::min(w.Bm, n - mpos);
+    const Levels ml = advance(lv, g, g.dense, false, mpos);  // the coarse levels from this middle span's first pair
+    int mlo = lo;
+    bool mbase = have_base;
+    for (int i = g.dense; i < mid_end; ++i)
+      if ((r = run_block(c, g, i, tk, mpos, mn, ml, mlo, mbase, st))) return r;
+    for (int pos = 0; pos < mn; pos += w.B) {
+      const int nb = std::min(w.B, mn - pos);
+      const Levels pl = advance(ml, g, mid_end, true, pos);  // every wider level and the planes from this pass's first pair
+      int plo = mlo;
+      bool pbase = mbase;
+      for (int i = mid_end; i < g.nb; ++i)
+        if ((r = run_block(c, g, i, tk, mpos + pos, nb, pl, plo, pbase, st))) return r;
+      span_begin(c, 90, st);
+      LAUNCH(launch_final((const float4*)c->imgs.p, pl.fs, plo, pbase ? pl.F : nullptr, pbase ? pl.M : nullptr,
+                          tk.batch(mpos + pos, nb), g.Hp, g.Wp, H, W, out + (size_t)(mpos + pos) * H * W * 3, st));
+      span_end(c, st);
+      c->last_fs = pl.fs;
+      c->last_F = pl.F;
+      c->last_M = pl.M;
+      c->last_lo = plo;
+      c->last_have_base = pbase;
+      c->ws_B = nb;
+    }
+  }
   return VFI_OK;
 }
 
@@ -617,7 +769,7 @@ int vfi_set_batch(vfi_ctx* c, int batch) {
 }
 
 // Per-group device times of the forward schedule: CUDA events on the launching stream around each kernel group of every
-// pass run while profiling is on (the groups and their ids are listed in forward_pass).  Off by default: the event
+// pass run while profiling is on (the groups and their ids are listed at span_begin).  Off by default: the event
 // records break the dependent-launch chaining between groups, so the timed bench steps run without it.
 int vfi_rife_profile(vfi_ctx* c, int enable) {
   if (!c) return fail(VFI_E_INVALID, "null ctx");
@@ -800,7 +952,8 @@ int vfi_rife46_forward(vfi_ctx* c, const float* frames, int n_frames, int H, int
     hi = std::max(hi, std::max(f0[i], f1[i]) + 1);
   }
   const int B = std::min(c->batch, n_tasks);
-  if ((r = ensure_workspace(c, g, B, hi - lo))) return r;
+  const Widths w = span_widths(c, g, B, n_tasks);
+  if ((r = ensure_workspace(c, g, w, hi - lo))) return r;
   cudaStream_t st = (cudaStream_t)stream;
   LAUNCH(launch_prep_frames(frames + (size_t)lo * H * W * C, hi - lo, H, W, C, (float4*)c->imgs.p, (uint2*)c->imgs_h.p,
                             g.Hp, g.Wp, st));
@@ -810,15 +963,14 @@ int vfi_rife46_forward(vfi_ctx* c, const float* frames, int n_frames, int H, int
       if ((r = run_encode(c, g, f, cnt, st))) return r;
     }
   }
-  for (int pos = 0; pos < n_tasks; pos += B) {
-    BatchTasks bt{};
-    bt.n = std::min(B, n_tasks - pos);
-    for (int i = 0; i < bt.n; ++i) {
-      bt.f0[i] = f0[pos + i] - lo;
-      bt.f1[i] = f1[pos + i] - lo;
-      bt.t[i] = t[pos + i];
-    }
-    if ((r = forward_pass(c, g, bt, H, W, out + (size_t)pos * H * W * 3, st))) return r;
+  std::vector<int32_t> w0(n_tasks), w1(n_tasks);  // frame indices into the prepared window
+  for (int i = 0; i < n_tasks; ++i) {
+    w0[i] = f0[i] - lo;
+    w1[i] = f1[i] - lo;
+  }
+  for (int pos = 0; pos < n_tasks; pos += w.Bc) {
+    const SpanTasks tk{w0.data() + pos, w1.data() + pos, t + pos};
+    if ((r = forward_span(c, g, tk, std::min(w.Bc, n_tasks - pos), w, H, W, out + (size_t)pos * H * W * 3, st))) return r;
   }
   return VFI_OK;
 }
@@ -896,7 +1048,8 @@ int vfi_rife46_interpolate_host(vfi_ctx* c, const float* frames, int n_frames, i
   int R = 1;
   for (int f = 0; f < nf; ++f)
     if (ctr[f] >= 0) R = std::max(R, up_end[std::min(last_pass[f] + 1, nb - 1)] - ctr[f]);
-  if ((r = ensure_workspace(c, g, B, R))) return r;
+  const Widths w{B, B, B, g.dense, -1};  // one pass per span: the upload ring sets the width
+  if ((r = ensure_workspace(c, g, w, R))) return r;
   const int kRaw = 2 * kMaxBatch + 4;  // raw upload ring (frames), overwritten in stream order on the copy stream
   CK(c->raw.ensure((size_t)kRaw * frame_bytes));
   CK(c->outdev.ensure((size_t)2 * B * out_bytes));
@@ -1090,15 +1243,13 @@ int vfi_rife46_interpolate_host(vfi_ctx* c, const float* frames, int n_frames, i
       CK(cudaEventRecord(ev_up[k], c->s_h2d));
       CK(cudaStreamWaitEvent(c->s_comp, ev_up[k], 0));
       if (k >= 2) CK(cudaStreamWaitEvent(c->s_comp, ev_down[k - 2], 0));  // output slot free again
-      BatchTasks bt{};
-      bt.n = n;
+      int32_t w0[kMaxBatch], w1[kMaxBatch];  // ring slots of the pass's frames
       for (int i = 0; i < n; ++i) {
-        bt.f0[i] = ctr[f0[pos + i] - frame_lo] % R;
-        bt.f1[i] = ctr[f1[pos + i] - frame_lo] % R;
-        bt.t[i] = t[pos + i];
+        w0[i] = ctr[f0[pos + i] - frame_lo] % R;
+        w1[i] = ctr[f1[pos + i] - frame_lo] % R;
       }
       float* od = (float*)c->outdev.p + (size_t)(k & 1) * B * out_elems;
-      int r2 = forward_pass(c, g, bt, H, W, od, c->s_comp);
+      int r2 = forward_span(c, g, SpanTasks{w0, w1, t + pos}, n, w, H, W, od, c->s_comp);
       if (r2) return r2;
       CK(cudaEventRecord(ev_comp[k], c->s_comp));
       CK(cudaStreamWaitEvent(c->s_d2h, ev_comp[k], 0));
@@ -1341,11 +1492,11 @@ int vfi_rife46_debug_state(vfi_ctx* c, float* flow4_out, float* mask_out, int ba
   CK(c->dbgF.ensure(n * sizeof(float4)));
   CK(c->dbgM.ensure(n * sizeof(float)));
   if (c->last_lo >= c->last_fs.n) {  // every level already folded into the dense planes (up-scaled last blocks)
-    CK(cudaMemcpy(c->dbgF.p, c->flow.p, n * sizeof(float4), cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(c->dbgM.p, c->mask.p, n * sizeof(float), cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(c->dbgF.p, c->last_F, n * sizeof(float4), cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(c->dbgM.p, c->last_M, n * sizeof(float), cudaMemcpyDeviceToDevice));
   } else {
-    LAUNCH(launch_materialize(c->last_fs, c->last_lo, c->last_have_base ? (const float4*)c->flow.p : nullptr,
-                              c->last_have_base ? (const float*)c->mask.p : nullptr, (float4*)c->dbgF.p,
+    LAUNCH(launch_materialize(c->last_fs, c->last_lo, c->last_have_base ? c->last_F : nullptr,
+                              c->last_have_base ? c->last_M : nullptr, (float4*)c->dbgF.p,
                               (float*)c->dbgM.p, batch, c->ws_Hp, c->ws_Wp, 0));
   }
   CK(cudaDeviceSynchronize());
