@@ -1,4 +1,4 @@
-"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR, IFRNet, CAIN) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
+"""H100-native drop-in for the RIFE (and FILM, Sepconv, GMFSS Fortuna, FLAVR, IFRNet, CAIN, IFUnet) path of Fannovel16/ComfyUI-Frame-Interpolation (ComfyUI custom-node package).
 
 Exports the same mapping names ComfyUI discovers in the reference's root __init__.py:23-47.
 """
@@ -9,6 +9,7 @@ from .gmfss_node import GMFSS_Fortuna_VFI  # noqa: F401
 from .flavr_node import FLAVR_VFI  # noqa: F401
 from .ifrnet_node import IFRNet_VFI  # noqa: F401
 from .cain_node import CAIN_VFI  # noqa: F401
+from .ifunet_node import IFUnet_VFI  # noqa: F401
 
 NODE_CLASS_MAPPINGS = {
     "RIFE VFI": RIFE_VFI,
@@ -18,6 +19,7 @@ NODE_CLASS_MAPPINGS = {
     "FLAVR VFI": FLAVR_VFI,
     "IFRNet VFI": IFRNet_VFI,
     "CAIN VFI": CAIN_VFI,
+    "IFUnet VFI": IFUnet_VFI,
     "Make Interpolation State List": MakeInterpolationStateList,
     "VFI FloatToInt": FloatToInt,
 }
@@ -30,4 +32,5 @@ NODE_DISPLAY_NAME_MAPPINGS = {
     "FLAVR VFI": "FLAVR VFI (H100 native)",
     "IFRNet VFI": "IFRNet VFI (H100 native)",
     "CAIN VFI": "CAIN VFI (H100 native)",
+    "IFUnet VFI": "IFUnet VFI (H100 native)",
 }

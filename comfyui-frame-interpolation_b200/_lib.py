@@ -22,6 +22,8 @@ SYMBOLS = [
     "vfi_ifrnet_layer_plan", "vfi_ifrnet_info", "vfi_streamconv_debug_conv", "vfi_streamconv_plan",
     "vfi_cain_load", "vfi_cain_forward", "vfi_cain_geometry", "vfi_cain_debug_set_ref", "vfi_cain_debug_conv",
     "vfi_cain_layer_plan", "vfi_cain_debug_elem",
+    "vfi_ifunet_load", "vfi_ifunet_forward", "vfi_ifunet_geometry", "vfi_ifunet_debug_set_ref", "vfi_ifunet_debug_conv",
+    "vfi_ifunet_layer_plan", "vfi_ifunet_debug_elem",
     # GMFSS building blocks (argtypes are set by gmfss.Ops)
     "vfi_gm_conv2d", "vfi_gm_conv2d_packed", "vfi_gm_transpose", "vfi_gm_convt4", "vfi_gm_instance_norm", "vfi_gm_layer_norm", "vfi_gm_softmax_rows", "vfi_gm_gemm", "vfi_gm_window", "vfi_gm_nchw_tokens", "vfi_gm_add_position", "vfi_gm_local_match", "vfi_gm_local_prop", "vfi_gm_convex_up", "vfi_gm_warp_zeros", "vfi_gm_resize", "vfi_gm_metric_input", "vfi_gm_pixel_shuffle2", "vfi_gm_axpby", "vfi_gm_copy_slice",
 ]
@@ -108,6 +110,13 @@ def lib():
     L.vfi_cain_debug_conv.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, vp]
     L.vfi_cain_layer_plan.argtypes = [vp, i32, vp, i32]
     L.vfi_cain_debug_elem.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, i32, vp]
+    L.vfi_ifunet_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]
+    L.vfi_ifunet_forward.argtypes = [vp, vp, vp, i32, i32, C.c_double, C.c_double, i32, vp, vp]
+    L.vfi_ifunet_geometry.argtypes = [i32, i32, C.c_double, vp, i32]
+    L.vfi_ifunet_debug_set_ref.argtypes = [vp, i32]
+    L.vfi_ifunet_debug_conv.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.vfi_ifunet_layer_plan.argtypes = [vp, i32, vp, i32]
+    L.vfi_ifunet_debug_elem.argtypes = [vp, i32, vp, vp, i32, i32, C.c_double, C.c_double, vp, vp, vp, i32, vp]
     L.vfi_streamconv_debug_conv.argtypes = [vp, i32, f32, i32, vp, vp, vp, vp, i32, vp, i32, vp, i32, vp, vp, i32, i32, i32,
                                             i32, i32, i32, vp]
     L.vfi_streamconv_plan.argtypes = [vp, i32, vp, i32]

@@ -208,6 +208,7 @@ struct vfi_ctx {
   vfi::ModelState* flavr = nullptr;  // FLAVR weights and workspace (flavr.cu)
   vfi::ModelState* ifrnet = nullptr;  // IFRNet weights and workspace (ifrnet.cu)
   vfi::ModelState* cain = nullptr;    // CAIN weights and workspace (cain.cu)
+  vfi::ModelState* ifunet = nullptr;  // IFUnet weights and workspace (ifunet.cu)
 };
 
 namespace vfi {
@@ -217,6 +218,7 @@ SepState*& ctx_sep(::vfi_ctx* c) { return c->sep; }
 ModelState*& ctx_flavr(::vfi_ctx* c) { return c->flavr; }
 ModelState*& ctx_ifrnet(::vfi_ctx* c) { return c->ifrnet; }
 ModelState*& ctx_cain(::vfi_ctx* c) { return c->cain; }
+ModelState*& ctx_ifunet(::vfi_ctx* c) { return c->ifunet; }
 void ctx_add_launches(::vfi_ctx* c, int n) { c->launches += n; }
 }  // namespace vfi
 
@@ -740,6 +742,8 @@ int vfi_destroy(vfi_ctx* c) {
   c->ifrnet = nullptr;
   delete c->cain;
   c->cain = nullptr;
+  delete c->ifunet;
+  c->ifunet = nullptr;
   c->film = nullptr;
   sepconv_destroy(c->sep);
   c->sep = nullptr;

@@ -340,6 +340,56 @@ cudaError_t launch_cain_apply(int op, const void* x, const float* g, const void*
 cudaError_t launch_cain_final(int op, const void* feat, int H, int W, int top, int left, int w, const double* partial,
                               float* out, cudaStream_t st);
 
+// ---- IFUnet kernels around the convolutions (ifunet_elem.cu); frames and output are fp32 [3][H][W] planes, padded
+// frames (Hp x Wp) read zeros beyond H x W; 16-bit tensors NHWC; flows fp32 ----
+constexpr int kIfuPoolChunks = 32;  // CBAM pool partials per image (a function of nothing but this constant)
+struct IfuFlowIn {                  // one IFUNet level input (launch_ifunet_flow_in)
+  const float* f0;
+  const float* f1;
+  int H, W, Hp, Wp;
+  const float* warped;  // [2][3][Hp][Wp] fp32, or null at level 0
+  const float* flow;    // [Hp][Wp][4] fp32, or null at level 0
+  int swap0;            // batch image 0 reads (img1, img0, 1 - t); image 1 always the opposite of image 0
+  float t;
+  int resize;           // scale != 1
+  float cscale, fscale; // coordinate scale (float)(1 / scale) and flow multiplier (float) scale
+  int h0, w0;           // the resized input's size
+  const float* c0w;     // level 0: conv0 weights [17][7], bias, PReLU slopes
+  const float* c0b;
+  const float* c0s;
+};
+cudaError_t launch_ifunet_flow_in(int op, const IfuFlowIn& a, int B, void* out, cudaStream_t st);
+cudaError_t launch_ifunet_s2d(int op, const void* in, int pitch, int cq, int B, int h, int w, void* out, int opitch,
+                              cudaStream_t st);
+cudaError_t launch_ifunet_d2s(const void* ph, int C, int B, int h, int w, void* out, cudaStream_t st);
+// CBAM in place on x [B][h][w][pitch] (C channels): mlp = {W1 [C/16][C], b1, W2 [C][C/16], b2}, sw = {7x7 weights
+// [2][49], bias} with BatchNorm folded; scratch psum / pmax [B][kIfuPoolChunks][C], gate [B][C], cmp [B][h][w][2]
+cudaError_t launch_ifunet_cbam(int op, void* x, int pitch, int C, int B, int h, int w, const float* mlp, const float* sw,
+                               float* psum, float* pmax, float* gate, float* cmp, cudaStream_t st);
+cudaError_t launch_ifunet_add16(int op, void* x, const void* y, size_t n, cudaStream_t st);
+cudaError_t launch_ifunet_convex(int op, const float* flow, const void* mask, int L, int B, int h, int w, float* up,
+                                 cudaStream_t st);
+cudaError_t launch_ifunet_flow_update(const float* up, int uh, int uw, int resize, float cscale, float fmul, int mode,
+                                      int Hp, int Wp, float* flow, cudaStream_t st);
+cudaError_t launch_ifunet_warp_frames(const float* f0, const float* f1, int H, int W, int Hp, int Wp, const float* flow,
+                                      float* warped, cudaStream_t st);
+cudaError_t launch_ifunet_fusion_in(int op, const float* f0, const float* f1, int H, int W, int Hp, int Wp,
+                                    const float* warped, const float* flow, void* out, cudaStream_t st);
+cudaError_t launch_ifunet_rrdb_res(int op, void* y, const void* x, size_t n, cudaStream_t st);
+cudaError_t launch_ifunet_merge(const float* warped, const float* last, int Hp, int Wp, float* deg, cudaStream_t st);
+cudaError_t launch_ifunet_fb_in(const float* f0, const float* f1, int H, int W, int Hp, int Wp, const float* deg,
+                                const float* rwarp, const float* rmask, const float* rflow, int cin, int s, float* out,
+                                cudaStream_t st);
+cudaError_t launch_ifunet_stem(int op, const float* src0, const float* src1, int cin, int sh, int sw, int vh, int vw,
+                               const float* w, const float* bias, const float* slopes, int cout, int B, int pitch, void* out,
+                               cudaStream_t st);
+cudaError_t launch_ifunet_fb_out(const float* ph, int h, int w, int s, int first, const float* f0, const float* f1, int H,
+                                 int W, int Hp, int Wp, float* rflow, float* rmask, float* rwarp, cudaStream_t st);
+cudaError_t launch_ifunet_ctx_warp(int op, const void* feat, int fpitch, const float* rflow, int Hp, int Wp, void* out,
+                                   cudaStream_t st);
+cudaError_t launch_ifunet_final(const float* ph, const float* rwarp, const float* rmask, const float* deg, int H, int W,
+                                int Hp, int Wp, float* out, cudaStream_t st);
+
 cudaError_t launch_adacof(const float* in, const float* weight, const float* off_i, const float* off_j, float* out, int N,
                           int C, int Hin, int Win, int F, int dil, int Ho, int Wo, cudaStream_t st);
 cudaError_t launch_edt_pass(const float* data, float* out, int bs, int h, int w, float diam2, cudaStream_t st);
@@ -364,6 +414,7 @@ FilmState*& ctx_film(::vfi_ctx* c);
 ModelState*& ctx_flavr(::vfi_ctx* c);  // a FlavrState (flavr.cu)
 ModelState*& ctx_ifrnet(::vfi_ctx* c);  // an IfrnetState (ifrnet.cu)
 ModelState*& ctx_cain(::vfi_ctx* c);    // a CainState (cain.cu)
+ModelState*& ctx_ifunet(::vfi_ctx* c);  // an IfunetState (ifunet.cu)
 SepState*& ctx_sep(::vfi_ctx* c);
 void ctx_add_launches(::vfi_ctx* c, int n);
 

@@ -775,3 +775,173 @@ class CainEngine:
 
     def sync(self):
         check(self._L.vfi_sync(self._ctx))
+
+
+# IFUNetModel().state_dict(): the flow net (FeatureNet UNet with CBAM, three IFBlocks), the RRDBNet fusion net and the
+# ResynNet refinement net, the unused DegCNN included (IFUNet_arch.py)
+def ifunet_state_dict_spec():
+    """IFUNetModel().state_dict() names and shapes, in order (608 tensors; num_batches_tracked are int64 scalars)."""
+    def conv_prelu(p, co, ci, k):
+        return [(p + "0.weight", (co, ci, k, k)), (p + "0.bias", (co,)), (p + "1.weight", (co,))]
+
+    def bn(p, c):
+        return [(p + n, (c,)) for n in ("weight", "bias", "running_mean", "running_var")] + [(p + "num_batches_tracked", ())]
+
+    def cbam(p, c):
+        return ([(p + "ChannelGate.mlp.1.weight", (c // 16, c)), (p + "ChannelGate.mlp.1.bias", (c // 16,)),
+                 (p + "ChannelGate.mlp.3.weight", (c, c // 16)), (p + "ChannelGate.mlp.3.bias", (c,)),
+                 (p + "SpatialGate.spatial.conv.weight", (1, 2, 7, 7))] + bn(p + "SpatialGate.spatial.bn.", 1))
+
+    def conv_bn(p, co, ci):
+        return [(p + "0.weight", (co, ci, 3, 3))] + bn(p + "1.", co) + [(p + "2.weight", (co,))]
+
+    f = "flownet.fmap."
+    s = conv_prelu(f + "conv0.", 17, 7, 1)
+    cin = 17
+    for i, co in enumerate((32, 64, 128, 256, 512)):
+        s += conv_prelu(f"{f}conv{i + 1}.conv1.", co, cin, 3) + conv_prelu(f"{f}conv{i + 1}.conv2.", co, co, 3)
+        s += cbam(f"{f}conv{i + 1}.cbam.", co) if i else []
+        cin = co
+    for lvl, ci, co in ((5, 512, 256), (4, 256, 128), (3, 128, 64)):
+        p = f"{f}deconv{lvl}."
+        s += [(p + "deconv.0.weight", (ci, ci // 2, 4, 4)), (p + "deconv.0.bias", (ci // 2,)),
+              (p + "deconv.1.weight", (ci // 2,))]
+        s += conv_prelu(p + "conv1.", ci // 2, ci, 3) + conv_prelu(p + "conv2.", co, ci // 2, 3)
+        s += cbam(p + "cbam.", co) if lvl == 5 else []
+    for b, c in enumerate((256, 128, 64)):
+        p = f"flownet.block{b}."
+        for j in range(6):
+            s += conv_prelu(f"{p}convblock.{j}.", c, c, 3)
+        s += [(p + "flowconv.weight", (4, c, 3, 3)), (p + "flowconv.bias", (4,))]
+        for L in (16, 8, 4):
+            s += [(f"{p}maskconvx{L}.weight", (L * L * 9, c, 1, 1)), (f"{p}maskconvx{L}.bias", (L * L * 9,))]
+    p = "fusionnet."
+    s += [(p + "conv_first.weight", (64, 16, 3, 3)), (p + "conv_first.bias", (64,))]
+    for r in range(6):
+        for d in range(1, 4):
+            q = f"{p}body.{r}.rdb{d}."
+            for k in range(1, 5):
+                s += [(f"{q}conv{k}.weight", (32, 32 + 32 * k, 3, 3)), (f"{q}conv{k}.bias", (32,))]
+            s += [(q + "conv5.weight", (64, 192, 3, 3)), (q + "conv5.bias", (64,))]
+    for n in ("conv_body", "conv_up1", "conv_up2", "conv_hr"):
+        s += [(f"{p}{n}.weight", (64, 64, 3, 3)), (f"{p}{n}.bias", (64,))]
+    s += [(p + "conv_last.weight", (1, 64, 3, 3)), (p + "conv_last.bias", (1,))]
+    for b, ci in enumerate((6, 12, 12)):
+        p = f"refinenet.block{b}."
+        s += conv_bn(p + "conv0.0.", 64, ci) + conv_bn(p + "conv0.1.", 128, 64) + conv_bn(p + "conv0.2.", 256, 128)
+        for j in range(6):
+            s += conv_bn(f"{p}convblock.{j}.", 256, 256)
+        s += [(p + "lastconv.weight", (256, 4, 4, 4)), (p + "lastconv.bias", (4,))]
+    p = "refinenet.degrad."
+    s += conv_prelu(p + "conv0.", 32, 3, 3)
+    for j in (1, 2, 3):
+        s += conv_prelu(f"{p}conv{j}.", 32, 32, 3)
+    s += [(p + "deconv.1.weight", (128, 32, 4, 4)), (p + "deconv.1.bias", (32,)), (p + "deconv.2.weight", (32,)),
+          (p + "deconv.3.weight", (3, 32, 3, 3)), (p + "deconv.3.bias", (3,))]
+    for c in (0, 1):
+        s += conv_prelu(f"refinenet.context{c}.0.", 16, 3, 3) + conv_prelu(f"refinenet.context{c}.1.", 32, 16, 3)
+    s += [("refinenet.decode.0.weight", (64, 32, 4, 4)), ("refinenet.decode.0.bias", (32,)),
+          ("refinenet.decode.1.weight", (32, 3, 4, 4)), ("refinenet.decode.1.bias", (3,))]
+    return s
+
+
+def ifunet_geometry(h: int, w: int, scale: float):
+    """The sizes vfi_ifunet_forward uses for an h x w frame at `scale`: the padded size and the flow net's input and its
+    five stride-2 levels; raises VfiError (a RuntimeError) where the reference raises."""
+    v = np.zeros(14, np.int32)
+    check(lib().vfi_ifunet_geometry(int(h), int(w), float(scale), v.ctypes.data, 14))
+    return dict(hp=int(v[0]), wp=int(v[1]), levels=[(int(v[2 + 2 * i]), int(v[3 + 2 * i])) for i in range(6)])
+
+
+class IfunetEngine:
+    """IFUnet (IFUNet.pth, IFUNetModel) on one H100: `state_dict` = the raw checkpoint; a missing or extra key and every
+    shape are refused, as the reference's strict load_state_dict refuses them.  fp16 operands with fp32 accumulation
+    ("float32", as the node runs it); flows, masks, gates and the output are fp32."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, dtype: str = "float32"):
+        if not torch.cuda.is_available():
+            raise VfiError("no CUDA device: this path has no CPU fallback")
+        if dtype not in OPERAND:
+            raise ValueError(f"dtype must be one of {list(OPERAND)}")
+        spec = ifunet_state_dict_spec()
+        names = {n for n, _ in spec}
+        extra = [k for k in state_dict if k not in names]
+        if extra:
+            raise KeyError(f"state_dict is not an IFUNet checkpoint; unexpected key {extra[0]}")
+        for name, shape in spec:
+            if name not in state_dict:
+                raise KeyError(f"state_dict is not an IFUNet checkpoint; missing {name}")
+            if tuple(state_dict[name].shape) != shape:
+                raise ValueError(f"IFUNet: {name} has shape {tuple(state_dict[name].shape)}, expected {shape}")
+        self._L = lib()
+        self.device = int(device)
+        self._ctx = C.c_void_p()
+        check(self._L.vfi_create(self.device, C.byref(self._ctx)))
+        hold = [state_dict[n].detach().to("cpu", torch.float32).reshape(-1).contiguous() for n, _ in spec]
+        ptrs = (C.c_void_p * len(hold))(*[t.data_ptr() for t in hold])
+        numel = (C.c_int64 * len(hold))(*[t.numel() for t in hold])
+        check(self._L.vfi_ifunet_load(self._ctx, ptrs, numel, len(hold), OPERAND[dtype]))
+        self.dtype = dtype
+
+    def close(self):
+        if getattr(self, "_ctx", None) is not None and self._ctx.value:
+            self._L.vfi_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def forward(self, img0: torch.Tensor, img1: torch.Tensor, timestep: float = 0.5, scale: float = 1.0,
+                ensemble: bool = True, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """img0, img1: CUDA float32 [1, 3, H, W] -> [1, 3, H, W] = model(img0, img1, timestep=timestep, scale=scale,
+        ensemble=ensemble).  Raises VfiError (a RuntimeError) before any launch where the reference raises."""
+        for x in (img0, img1):
+            assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4 and x.shape[:2] == (1, 3)
+        assert img0.shape == img1.shape
+        _, _, h, w = img0.shape
+        if out is None:
+            out = torch.empty((1, 3, h, w), dtype=torch.float32, device=img0.device)
+        assert out.is_cuda and out.is_contiguous() and out.dtype == torch.float32 and out.shape == img0.shape
+        st = torch.cuda.current_stream(img0.device).cuda_stream
+        check(self._L.vfi_ifunet_forward(self._ctx, img0.data_ptr(), img1.data_ptr(), h, w, float(timestep), float(scale),
+                                         1 if ensemble else 0, out.data_ptr(), st))
+        return out
+
+    # ------------------------------------------------------------------ hooks
+    def set_ref(self, use_ref: bool):
+        check(self._L.vfi_ifunet_debug_set_ref(self._ctx, 1 if use_ref else 0))
+
+    def debug_conv(self, layer, src0, pitch0, src1, pitch1, out, out_pitch, B, H, W, impl=0, res=None, out_f32=None,
+                   f32_pitch=0):
+        """One conv layer on raw 16-bit NHWC tensors (pointers with element offsets already applied)."""
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        st = torch.cuda.current_stream(src0.device).cuda_stream
+        check(self._L.vfi_ifunet_debug_conv(self._ctx, layer, p(src0), int(pitch0), p(src1), int(pitch1), p(out),
+                                            int(out_pitch), p(res), p(out_f32), int(f32_pitch), B, H, W, impl, st))
+        return out
+
+    def layer_plan(self, layer):
+        v = np.zeros(14, np.int32)
+        check(self._L.vfi_ifunet_layer_plan(self._ctx, layer, v.ctypes.data, 14))
+        keys = ("c0", "c1", "n_total", "ksize", "act", "ext", "n_f32", "pad_before", "pad_before_x", "n_cta", "nsplit",
+                "a_slots", "b_slots", "smem_bytes")
+        return dict(zip(keys, [int(x) for x in v]))
+
+    def debug_elem(self, kernel, H, W, img0=None, img1=None, x=None, y=None, out=None, index=0, timestep=0.5,
+                   scale=1.0):
+        """One element-wise stage (vfi_ifunet_debug_elem): 0 the level-0 input of `index` images, 1 CBAM `index` in
+        place on out, 2 the convex upsampling of IFBlock `index`, 3 the warps of a pair."""
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        check(self._L.vfi_ifunet_debug_elem(self._ctx, kernel, p(img0), p(img1), H, W, float(timestep), float(scale),
+                                            p(x), p(y), p(out), index, st))
+        return out
+
+    def launch_count(self) -> int:
+        return int(self._L.vfi_launch_count(self._ctx))
+
+    def sync(self):
+        check(self._L.vfi_sync(self._ctx))

@@ -299,6 +299,37 @@ int vfi_cain_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
 int vfi_cain_debug_elem(vfi_ctx* ctx, int kernel, const float* img0, const float* img1, int H, int W, const void* x,
                         const void* res, void* out, int rcab, void* stream);
 
+/* IFUnet (`IFUnet VFI` node: IFUNetModel, IFUNet.pth) ------------------------------------------------------- */
+#define VFI_IFUNET_NUM_TENSORS 608
+/* Replaces: IFUNetModel().load_state_dict(torch.load(path)) (ifunet/__init__.py).  HOST float32 arrays in state_dict()
+ * order (engine.py ifunet_state_dict_spec; the num_batches_tracked scalars and the unused refinenet.degrad tensors
+ * included); every tensor's size is checked and a refusal names the tensor.  Eval-mode BatchNorm is folded at load. */
+int vfi_ifunet_load(vfi_ctx* ctx, const float* const* tensors, const int64_t* numel, int n_tensors, int operand_type);
+/* Replaces: `model(img0, img1, timestep=t, scale=scale, ensemble=ensemble)` for one pair (IFUNetModel.forward).
+ * DEVICE pointers: img0, img1 and out are float32 [3][H][W] planes (NCHW, batch 1).  A scale at which the reference
+ * raises (a UpConv input that does not double to its skip connection, or a level's flow that does not come back to the
+ * padded size) and a workspace the device cannot hold are refused before any launch.  Asynchronous on `stream`. */
+int vfi_ifunet_forward(vfi_ctx* ctx, const float* img0, const float* img1, int H, int W, double timestep, double scale,
+                       int ensemble, float* out, void* stream);
+/* The sizes vfi_ifunet_forward would use (no context): {Hp, Wp, then h, w of the flow net's input and of its five
+ * stride-2 levels} (14 values), or the error it would return. */
+int vfi_ifunet_geometry(int H, int W, double scale, int32_t* info, int cap);
+/* Test hooks: every conv through the CUDA-core checker (1) / the wgmma kernel (0); run one conv layer (ids in
+ * csrc/ifunet.cu) on 16-bit NHWC slices, with its residual and fp32 columns; its plan {c0, c1, n_total, ksize, act,
+ * ext, n_f32, pad_before, pad_before_x, n_cta, nsplit, a_slots, b_slots, smem_bytes}.  vfi_ifunet_debug_elem runs one
+ * element-wise stage on DEVICE tensors: kernel 0 the level-0 input of `index` (1 or 2) images of an H x W pair at
+ * `scale` / `timestep` (img0, img1 -> out, the 128-channel space-to-depth copy), 1 CBAM `index` (0..3: FeatureNet conv2
+ * .. conv5, 4: deconv5) in place on out [H][W][C], 2 the convex upsampling of IFBlock `index` (x: flow fp32 [H][W][4],
+ * y: mask logits [H][W][9 L L] 16-bit -> out fp32 [L H][L W][4]), 3 the warps of an H x W pair by x = flow fp32
+ * [Hp][Wp][4] -> out fp32 [2][3][Hp][Wp].  Asynchronous on `stream`. */
+int vfi_ifunet_debug_set_ref(vfi_ctx* ctx, int use_ref);
+int vfi_ifunet_debug_conv(vfi_ctx* ctx, int layer, const void* src0, int pitch0, const void* src1, int pitch1, void* out,
+                          int out_pitch, const void* res, float* out_f32, int f32_pitch, int B, int H, int W, int impl,
+                          void* stream);
+int vfi_ifunet_layer_plan(vfi_ctx* ctx, int layer, int32_t* info, int cap);
+int vfi_ifunet_debug_elem(vfi_ctx* ctx, int kernel, const float* img0, const float* img1, int H, int W, double timestep,
+                          double scale, const void* x, const void* y, void* out, int index, void* stream);
+
 /* Test / profiling hooks (used by tests/ and bench.py only) --------------------------------------------- */
 /* Run ONE convolution layer of block `block` (0..3; arch 4.26: 0..4): layer 0 = conv0.0, 1 = conv0.1, 2..9 = ResConv
  * 0..7, 10 = lastconv (flow + mask), 11 = arch 4.26 blocks 0..3: the 8 feature channels of lastconv, written as
