@@ -11,6 +11,7 @@ SYMBOLS = [
     "vfi_rife46_load", "vfi_rife_load", "vfi_rife46_forward", "vfi_rife46_interpolate_host", "vfi_warp_bilinear_border",
     "vfi_softsplat_sum", "vfi_softsplat_weighted", "vfi_costvol_l1", "vfi_corr_dot", "vfi_sepconv", "vfi_adacof", "vfi_edt_pass",
     "vfi_rife46_debug_layer", "vfi_rife46_debug_state", "vfi_rife46_layer_plan", "vfi_sync",
+    "vfi_rife46_debug_conv0_fused", "vfi_rife46_debug_unfused_conv0", "vfi_rife46_conv0_plan",
     "vfi_rife_profile", "vfi_rife_profile_read", "vfi_host_copy_frames",
     "vfi_film_load", "vfi_film_forward", "vfi_film_debug_set_ref", "vfi_film_debug_conv", "vfi_film_layer_plan",
     "vfi_film_last_macs", "vfi_film_debug_pack_host", "vfi_film_debug_state", "vfi_film_debug_elem",
@@ -68,6 +69,9 @@ def lib():
     L.vfi_rife46_debug_state.argtypes = [vp, vp, vp, i32, C.POINTER(i32), C.POINTER(i32)]
     L.vfi_rife46_layer_plan.argtypes = [vp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
                                         C.POINTER(i32), C.POINTER(i64), C.POINTER(i32), C.POINTER(i32)]
+    L.vfi_rife46_debug_conv0_fused.argtypes = [vp, i32, vp, vp, i32, i32, i32, vp]
+    L.vfi_rife46_debug_unfused_conv0.argtypes = [vp, i32]
+    L.vfi_rife46_conv0_plan.argtypes = [vp, i32, vp, i32]
     L.vfi_sync.argtypes = [vp]
     L.vfi_rife_profile.argtypes = [vp, i32]
     L.vfi_host_copy_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32]

@@ -96,6 +96,9 @@ __device__ __forceinline__ void bulk_wait() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 // 8x8 16-bit matrices, one 16-byte row address per lane (lanes 8 i .. 8 i + 7: matrix i); thread t holds row t / 4,
 // columns 2 (t % 4), +1 of matrix i in register i - the wgmma accumulator fragment layout of 8 rows x 8 columns
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t* r) {

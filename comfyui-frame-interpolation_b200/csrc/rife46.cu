@@ -7,6 +7,7 @@
 //     front      -> x      [B, Hs/2, Ws/2, 4*16]  16-bit      warp+concat+1/s       :31-70,:238-249,:589-596
 //     tapconv    -> c00    [B, Hs/4, Ws/4, 4*c/2] 16-bit      conv0.0 (+lrelu)      :181-184
 //     tapconv    -> feat   [B, Hs/4, Ws/4, c]     16-bit      conv0.1 (+lrelu)
+//                (4.6's full-resolution block: conv0.0 + conv0.1 as one launch, c00 stays on the SM)
 //     8x tapconv -> feat                                       ResConv               :20-28
 //     tapconv    -> tmp    [B, Hs, Ws] float4 + float          ConvT+PixelShuffle    :215-218
 //     (flow(p) = F(p) + sum_j up(T_j)(p)*s_j: F is stored only by fronts that visit every pixel)  :263-266,:694-696
@@ -209,6 +210,7 @@ struct vfi_ctx {
   vfi::ModelState* ifrnet = nullptr;  // IFRNet weights and workspace (ifrnet.cu)
   vfi::ModelState* cain = nullptr;    // CAIN weights and workspace (cain.cu)
   vfi::ModelState* ifunet = nullptr;  // IFUnet weights and workspace (ifunet.cu)
+  bool conv0_unfused = false;  // test hook (vfi_rife46_debug_unfused_conv0): conv0.0 and conv0.1 always as two launches
 };
 
 namespace vfi {
@@ -507,7 +509,16 @@ int run_encode(vfi_ctx* c, const Geometry& g, int f, int n, cudaStream_t st) {
   return VFI_OK;
 }
 
+// Whether block i runs conv0.0 and conv0.1 as one launch (launch_conv0_fused): arch 4.6's 64-channel block at full
+// resolution, the block whose conv0.0 output is too large to stay in L2 between two launches.  Elsewhere that output is
+// small and largely L2-resident, and the 128-channel block inputs of the other archs do not fit the fused kernel's window.
+bool conv0_fused(const vfi_ctx* c, const Geometry& g, int i) {
+  return !c->conv0_unfused && c->arch == 46 && g.s[i] == 1 && g.k[i] == 1 &&
+         conv0_fused_plan(c->layers[i][LAYER_CONV00], c->layers[i][LAYER_CONV01], c->op_type, nullptr, nullptr, nullptr) > 0;
+}
+
 // group ids of vfi_rife_profile: 10 * block + {0 front, 1 conv0.0, 2 conv0.1, 3 the 8 ResConvs, 4 lastconv(s)}, 90 final.
+// A block that runs conv0.0 and conv0.1 as one launch records it as group 10 * block + 1 and has no group 10 * block + 2.
 // A coarse block's spans cover its whole coarse span of pairs, a dense block's one pass.
 void span_begin(vfi_ctx* c, int id, cudaStream_t st) {
   if (!c->profile) return;
@@ -608,13 +619,19 @@ int run_block(vfi_ctx* c, const Geometry& g, int i, const SpanTasks& tk, int pos
   }
   span_end(c, st);
   span_begin(c, 10 * i + 1, st);
-  LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV00], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, n, Hs / 2, Ws / 2,
-                        c->num_sms, TAPCONV_PLANNED, st));
-  span_end(c, st);
-  span_begin(c, 10 * i + 2, st);
-  LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV01], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, n, Hs / 4, Ws / 4,
-                        c->num_sms, TAPCONV_PLANNED, st));
-  span_end(c, st);
+  if (conv0_fused(c, g, i)) {
+    LAUNCH(launch_conv0_fused(c->layers[i][LAYER_CONV00], c->layers[i][LAYER_CONV01], c->op_type, c->x.p, c->c00.p,
+                              c->featA.p, n, Hs / 2, Ws / 2, c->num_sms, st));
+    span_end(c, st);
+  } else {
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV00], c->op_type, c->x.p, c->c00.p, nullptr, nullptr, n, Hs / 2, Ws / 2,
+                          c->num_sms, TAPCONV_PLANNED, st));
+    span_end(c, st);
+    span_begin(c, 10 * i + 2, st);
+    LAUNCH(launch_tapconv(c->layers[i][LAYER_CONV01], c->op_type, c->c00.p, c->featA.p, nullptr, nullptr, n, Hs / 4,
+                          Ws / 4, c->num_sms, TAPCONV_PLANNED, st));
+    span_end(c, st);
+  }
   void* a = c->featA.p;
   void* b = c->featB.p;
   span_begin(c, 10 * i + 3, st);
@@ -1483,6 +1500,25 @@ int vfi_rife46_debug_layer(vfi_ctx* c, int block, int layer, const void* in, voi
   return VFI_OK;
 }
 
+int vfi_rife46_debug_conv0_fused(vfi_ctx* c, int block, const void* in, void* out, int B, int H, int W, void* stream) {
+  if (!c || block < 0 || !in || !out) return fail(VFI_E_INVALID, "bad argument");
+  if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
+  if (!block_has_layer(c->arch, block, LAYER_CONV01)) return fail(VFI_E_INVALID, "no such block in the loaded arch");
+  const TapConvLayer& L0 = c->layers[block][LAYER_CONV00];
+  const TapConvLayer& L1 = c->layers[block][LAYER_CONV01];
+  if (c->arch != 46 || conv0_fused_plan(L0, L1, c->op_type, nullptr, nullptr, nullptr) < 1)
+    return fail(VFI_E_INVALID, "this block's conv0.0 / conv0.1 do not run as one launch");
+  CK(cudaSetDevice(c->device));
+  LAUNCH(launch_conv0_fused(L0, L1, c->op_type, in, nullptr, out, B, H, W, c->num_sms, (cudaStream_t)stream));
+  return VFI_OK;
+}
+
+int vfi_rife46_debug_unfused_conv0(vfi_ctx* c, int unfused) {
+  if (!c) return fail(VFI_E_INVALID, "null context");
+  c->conv0_unfused = unfused != 0;
+  return VFI_OK;
+}
+
 int vfi_rife46_debug_state(vfi_ctx* c, float* flow4_out, float* mask_out, int batch, int* Hp, int* Wp) {
   if (!c || !Hp || !Wp) return fail(VFI_E_INVALID, "null argument");
   CK(cudaSetDevice(c->device));
@@ -1525,6 +1561,24 @@ int vfi_rife46_layer_plan(vfi_ctx* c, int block, int layer, int* stages, int* n_
   if (macs_per_cell) *macs_per_cell = (int64_t)(L.wstream ? 9 * L.cin : L.ktotal16 * 16) * L.n_total;
   if (cmajor) *cmajor = p.cmajor;
   if (wstream) *wstream = p.wstream;
+  return VFI_OK;
+}
+
+int vfi_rife46_conv0_plan(vfi_ctx* c, int block, int32_t* info, int cap) {
+  if (!c || block < 0 || (!info && cap > 0)) return fail(VFI_E_INVALID, "bad argument");
+  if (!c->loaded) return fail(VFI_E_STATE, "vfi_rife46_load has not been called");
+  if (!block_has_layer(c->arch, block, LAYER_CONV01)) return fail(VFI_E_INVALID, "no such block in the loaded arch");
+  int32_t v[5] = {0, 0, 0, 0, 0};
+  if (c->arch == 46) {
+    int smem = 0, regs = 0, local = 0;
+    v[1] = conv0_fused_plan(c->layers[block][LAYER_CONV00], c->layers[block][LAYER_CONV01], c->op_type, &smem, &regs,
+                            &local);
+    v[0] = v[1] > 0 ? 1 : 0;
+    v[2] = smem;
+    v[3] = regs;
+    v[4] = local;
+  }
+  for (int k = 0; k < cap && k < 5; ++k) info[k] = v[k];
   return VFI_OK;
 }
 

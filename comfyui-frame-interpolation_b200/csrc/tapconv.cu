@@ -88,6 +88,8 @@ __device__ __forceinline__ size_t out_pixel_offset(const TapConvParams& p, int b
 // box row is 128 / 64 / 32 bytes and uses the swizzle of that width (conflict-free stmatrix into the staging tile).
 __host__ __device__ constexpr int store_box_c(int n_cta) { return n_cta % 64 == 0 ? 64 : n_cta % 32 == 0 ? 32 : 16; }
 
+uint32_t align_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
+
 #ifndef VFI_HOST_EMU  // (tests/host_emu runs the RIFE schedule on the CPU with the checker kernel; no wgmma there)
 // Byte offset of 16-byte chunk `chunk` of row `row` in a 1024-aligned region of rowb-byte rows (32, 64 or 128) laid out
 // by TMA with the swizzle of that width: address bits [4, 4 + log2(rowb / 16)) are XORed with bits [7, ...).
@@ -100,7 +102,8 @@ __device__ __forceinline__ uint32_t swz_off(uint32_t row, uint32_t chunk, uint32
 // instead of two integer divisions per tile and role.
 struct TileIter {
   int b, ty, tx, db, dy, dx, tiles_x, tiles_y;
-  __device__ __forceinline__ TileIter(const TapConvParams& p, int first, int step) {
+  template <class P>
+  __device__ __forceinline__ TileIter(const P& p, int first, int step) {
     tiles_x = p.tiles_x;
     tiles_y = p.tiles_y;
     const int per_img = tiles_x * tiles_y;
@@ -184,6 +187,36 @@ __device__ __forceinline__ void issue_wslot(const TapConvParams& p, float (&acc)
     for (int h = 0; h < 2; ++h)
       wgmma_ss<N, T>(acc[h], ((uint64_t)d.y << 32) | (uint64_t)(a_base + d.x + (uint32_t)h * half_off), b64,
                      j ? 1u : 0u);
+  }
+}
+
+// Staged 16-bit output of one 64-row accumulator half: this warp's tile rows `row` and `row + 1` (d[4 j + 2 e + c] = tile
+// row row + e, column lane / 4, channel 8 j + c2 + c), through max(a, slope * a) and rounded to 16 bits, stmatrix'ed into
+// a staging tile of N / store_box_c(N) boxes of box_bytes each, swizzled like the box rows.
+template <int N, typename T>
+__device__ __forceinline__ void stage_rows(const float (&a)[N / 2], uint32_t out_smem, uint32_t box_bytes, int row, int lane,
+                                           float slope) {
+  constexpr int kBoxC = store_box_c(N);
+  constexpr uint32_t kBoxRow = 2u * kBoxC;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const uint32_t pix = (uint32_t)((row + e) * kTileW + (lane & 7));
+#pragma unroll
+    for (int jb = 0; jb < N / 8; jb += 4) {
+      const bool x4 = N / 8 - jb >= 4;
+      const int col = 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
+      const uint32_t addr = out_smem + (uint32_t)(col / kBoxC) * box_bytes + swz_off(pix, (uint32_t)(col % kBoxC) >> 3, kBoxRow);
+      uint32_t r[4];
+#pragma unroll
+      for (int i = 0; i < (x4 ? 4 : 2); ++i) {
+        const float a0 = a[4 * (jb + i) + 2 * e], a1 = a[4 * (jb + i) + 2 * e + 1];
+        r[i] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
+      }
+      if (x4)
+        stsm_x4(addr, r);
+      else
+        stsm_x2(addr, r);
+    }
   }
 }
 
@@ -487,28 +520,7 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
           }
       } else {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const uint32_t pix = (uint32_t)((8 * h + 2 * wq + e) * kTileW + (lane & 7));
-#pragma unroll
-            for (int jb = 0; jb < N / 8; jb += 4) {
-              const bool x4 = N / 8 - jb >= 4;
-              const int col = 8 * (jb + (x4 ? (lane >> 3) : ((lane >> 3) & 1)));
-              const uint32_t addr =
-                  out_smem + (uint32_t)(col / kBoxC) * kBoxBytes + swz_off(pix, (uint32_t)(col % kBoxC) >> 3, kBoxRow);
-              uint32_t r[4];
-#pragma unroll
-              for (int i = 0; i < (x4 ? 4 : 2); ++i) {
-                const float a0 = acc[h][4 * (jb + i) + 2 * e], a1 = acc[h][4 * (jb + i) + 2 * e + 1];
-                r[i] = Pack2<T>::pack(fmaxf(a0, slope * a0), fmaxf(a1, slope * a1));
-              }
-              if (x4)
-                stsm_x4(addr, r);
-              else
-                stsm_x2(addr, r);
-            }
-          }
+        for (int h = 0; h < 2; ++h) stage_rows<N, T>(acc[h], out_smem, kBoxBytes, 8 * h + 2 * wq, lane, slope);
       }
       fence_proxy_async();  // the generic-proxy staging writes before the TMA engine reads them
       named_bar_sync(1 + g, 128);
@@ -586,6 +598,228 @@ __global__ void __launch_bounds__(WS ? kThreadsWS : kThreads, 1) tapconv_kernel(
   if (tma_out && leader) bulk_wait<0>();  // the CTA's last stores have landed before it exits
 }
 
+#endif  // VFI_HOST_EMU
+
+// ---------------------------------------------------------------------------------------------
+// conv0.0 -> conv0.1 of a full-resolution arch-4.6 block as one launch (conv0_fused_kernel): conv0.0's output never
+// leaves the SM.  One tile = 8 x 8 conv0.1 outputs (quarter-resolution cells).  conv0.1 reads the 9 x 9 conv0.0 cells
+// [y0 - 1, y0 + 7] x [x0 - 1, x0 + 7] (its stride-2 taps are dy, dx in {-1, 0}), i.e. 18 x 18 conv0.0 outputs in
+// space-to-depth form, which read the 19 x 19 block-input cells from (2 y0 - 3, 2 x0 - 3): one TMA box, zero-filled
+// outside the image as for the unfused conv0.0.
+//   conv0.0 runs cell-major on that window taken as ONE row of kC0XW-cell rows: output (wr, wc) of the window
+//   (1 <= wr, wc <= 18) is window row L = wr * kC0XW + wc, and its tap (dy, dx) window row L + dy * kC0XW + dx, so each
+//   m64n32 MMA covers 64 consecutive L (SBO = 8 rows x 128 B) and kC0MB of them cover L in [kC0XW + 1, 18 kC0XW + 18]
+//   (the wc = 0 column and the rows read past the loaded box give outputs that are dropped).  Its epilogue (shift,
+//   LeakyReLU, 16-bit) writes the conv0.1 window exactly as TMA would have staged conv0.0's space-to-depth output: two
+//   SWIZZLE_128B k-blocks (sub-rows 0 and 1) of 9 x 9 cells x 128 B, and zeros for cells outside the grid (conv0.1's
+//   padding).  conv0.1 then runs its planned tap descriptors on that window (one m64 row block) and leaves through the
+//   staged TMA store.  Same products in the same K order into fp32 and the same roundings as the two launches.
+// Shared memory: control block, both layers' weights (resident for the launch), and per MMA warpgroup its x window, its
+// conv0.1 window and its output staging tile.  Warpgroup g takes the CTA's tiles g, g + 2, ...; the producer refills a
+// warpgroup's x window as soon as that warpgroup's conv0.0 MMAs have read it, so one fill is in flight while both compute.
+constexpr int kC0XW = 19;                                // x window: 19 x 19 cells of 64 channels (128 B)
+constexpr int kC0MB = 6;                                 // conv0.0 m64 row blocks: L in [20, 20 + 384)
+constexpr uint32_t kC0XBox = kC0XW * kC0XW * 128u;       // TMA bytes of one x window
+constexpr uint32_t kC0XBytes = (kC0XW + 1 + 64 * kC0MB) * 128u;  // rows the conv0.0 MMAs address (past the box: unused)
+constexpr int kC0Tile = 8;                               // conv0.1 tile: 8 x 8 cells
+constexpr uint32_t kC0OutBytes = kC0Tile * kC0Tile * 128u;  // 64 channels x 16 bit per cell
+
+struct alignas(64) Conv0Params {
+  CUtensorMap tm_x;    // block input {64, W2, H2, B}, box {64, 19, 19, 1}, SWIZZLE_128B
+  CUtensorMap tm_out;  // conv0.1 output {64, W4, H4, B}, box {64, 8, 8, 1}, SWIZZLE_128B
+  const void* w0;      // conv0.0 / conv0.1 packed weights and shifts (their TapConvLayers)
+  const void* w1;
+  const float* shift0;
+  const float* shift1;
+  int B, H4, W4;  // conv0.1 grid (conv0.0's: 2 H4 x 2 W4)
+  int tiles_x, tiles_y, ntiles, ctas;
+  uint32_t w0_bytes, w1_bytes;
+  uint32_t off_w0, off_w1, off_wg, wg_bytes, off_c00, c00_kb1, off_out, smem_bytes;
+  uint32_t b_hi;  // weight (B) descriptor high word of both layers
+  uint4 mma0[9];  // conv0.0 steps {A offset from the x window, A high word, B offset, 0}, 16-byte units
+  uint4 mma1[9];  // conv0.1 runs of two steps {A offset from the conv0.1 window, A high word, B offset, 0}
+};
+
+// Both layers' shapes as the kernel hard-codes them: conv0.0 64 -> 32 channels as 9 one-step taps, conv0.1 128 -> 64 as
+// 9 two-step runs, each in one output-channel split.  Fills the shared-memory layout and descriptors; false otherwise.
+bool conv0_fused_layout(const TapConvLayer& L0, const TapConvLayer& L1, Conv0Params* pp) {
+  Conv0Params& p = *pp;
+  if (L0.cin != 64 || L0.n_total != 32 || L0.nsplit != 1 || L0.ntaps != 9 || L0.ktotal16 != 9 || L0.out_s2d != 1 ||
+      L0.epi_mode != EPI_BIAS_LRELU || L1.cin != 128 || L1.n_total != 64 || L1.nsplit != 1 || L1.out_s2d != 0 ||
+      L1.epi_mode != EPI_BIAS_LRELU || L1.halo_y0 != -1 || L1.halo_x0 != -1 || L1.halo_w != kC0Tile + 1)
+    return false;
+  for (int e = 0; e < 9; ++e)
+    if (L0.taps[e].nk16 != 1 || L0.taps[e].dy < -1 || L0.taps[e].dy > 0 || L0.taps[e].dx < -1 || L0.taps[e].dx > 0)
+      return false;
+  // conv0.1's window: its layer planned over a 9-row window (the descriptors depend on the rows only through kb_off)
+  TapConvLayer L1w = L1;
+  L1w.halo_h = kC0Tile + 1;
+  TapConvParams q{};
+  if (tapconv_plan(L1w, &q) < 1 || q.nkb != 2 || q.nruns != 9 || q.run_len != 2) return false;
+  p.w0_bytes = 3u * 32u * 128u;  // ceil(9 / 4) rows of four K=16 steps x 32 columns
+  p.w1_bytes = q.w_bytes;
+  p.b_hi = q.b_hi;
+  for (int r = 0; r < 9; ++r) p.mma1[r] = q.mma[r];
+  p.c00_kb1 = q.kb_off[1];
+  for (int j = 0; j < 9; ++j) {
+    const TapEntry te = L0.taps[j];
+    const uint32_t a_off = (uint32_t)(kC0XW + 1 + te.dy * kC0XW + te.dx) * 128u + (uint32_t)te.chunk0 * 16u;
+    const uint32_t b_off = (uint32_t)(j >> 2) * (32u * 128u) + (uint32_t)(j & 3) * 32u;
+    p.mma0[j] = make_uint4(a_off >> 4, (1024u >> 4) | kDescSw128, b_off >> 4, 0u);
+  }
+  p.off_w0 = align_up(kCtrlBytes, 1024);
+  p.off_w1 = align_up(p.off_w0 + p.w0_bytes, 1024);
+  p.off_wg = align_up(p.off_w1 + p.w1_bytes, 1024);
+  p.off_c00 = align_up(kC0XBytes, 1024);
+  p.off_out = p.off_c00 + q.stage_bytes;
+  p.wg_bytes = p.off_out + kC0OutBytes;
+  p.smem_bytes = p.off_wg + (uint32_t)kMmaGroups * p.wg_bytes;
+  return p.smem_bytes <= (uint32_t)kSmemLimit;
+}
+
+#ifndef VFI_HOST_EMU
+template <typename T>
+__global__ void __launch_bounds__(kThreads, 1) conv0_fused_kernel(const __grid_constant__ Conv0Params p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  asm volatile("griddepcontrol.launch_dependents;");  // (programmatic dependent launch, as tapconv_kernel)
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int first = (int)blockIdx.x;
+  const int tstep = p.ctas;
+  const int my_tiles = (p.ntiles - first + tstep - 1) / tstep;
+  const uint32_t smem_base = smem_u32(smem);
+  // control block: weights full, then per warpgroup its x window's "full" and "empty" barriers
+  const uint32_t bar_w = smem_base, bar_full = smem_base + 8, bar_empty = smem_base + 8 + 8 * kMmaGroups;
+  const uint32_t w0_smem = smem_base + p.off_w0, w1_smem = smem_base + p.off_w1;
+  if (threadIdx.x == 0) {
+    mbar_init(bar_w, 1);
+    for (int g = 0; g < kMmaGroups; ++g) {
+      mbar_init(bar_full + 8 * g, 1);
+      mbar_init(bar_empty + 8 * g, 4);  // the four warps of the warpgroup
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp == kTmaWarp) {
+    if (lane == 0) {
+      mbar_arrive_expect_tx(bar_w, p.w0_bytes + p.w1_bytes);
+      bulk_g2s(w0_smem, p.w0, p.w0_bytes, bar_w);
+      for (uint32_t off = 0; off < p.w1_bytes; off += 32768u)
+        bulk_g2s(w1_smem + off, reinterpret_cast<const uint8_t*>(p.w1) + off, min(32768u, p.w1_bytes - off), bar_w);
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      TileIter it(p, first, tstep);
+      // bit g: parity of the next "empty" wait on warpgroup g's window (1: the first fill of each window needs no wait)
+      uint32_t eph = (1u << kMmaGroups) - 1u;
+      for (int k = 0; k < my_tiles; ++k, it.next()) {
+        const int g = k & 1;
+        mbar_wait(bar_empty + 8 * g, (eph >> g) & 1u);
+        eph ^= 1u << g;
+        mbar_arrive_expect_tx(bar_full + 8 * g, kC0XBox);
+        tma_load_4d(smem_base + p.off_wg + (uint32_t)g * p.wg_bytes, &p.tm_x, bar_full + 8 * g, 0,
+                    2 * kC0Tile * it.tx - 3, 2 * kC0Tile * it.ty - 3, it.b);
+      }
+    }
+    return;
+  }
+
+  const int g = warp >> 2;
+  const int wq = warp & 3;
+  const int px = lane >> 2;
+  const int c2 = 2 * (lane & 3);
+  float2 sh0[4], sh1[8];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) sh0[j] = __ldg(reinterpret_cast<const float2*>(p.shift0 + 8 * j + c2));
+#pragma unroll
+  for (int j = 0; j < 8; ++j) sh1[j] = __ldg(reinterpret_cast<const float2*>(p.shift1 + 8 * j + c2));
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  mbar_wait(bar_w, 0);
+  const uint32_t region = smem_base + p.off_wg + (uint32_t)g * p.wg_bytes;
+  const uint32_t c00 = region + p.off_c00, out_smem = region + p.off_out;
+  const uint32_t x_lo = (1u << 16) | (region >> 4), c00_lo = (1u << 16) | (c00 >> 4);
+  const uint32_t b0_lo = (1u << 16) | (w0_smem >> 4), b1_lo = (1u << 16) | (w1_smem >> 4);
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int H2 = 2 * p.H4, W2 = 2 * p.W4;
+  uint32_t fph = 0;
+  float acc0[kC0MB][16];
+  float acc1[32];
+
+  TileIter it(p, first + g * tstep, kMmaGroups * tstep);
+  for (int k = g; k < my_tiles; k += kMmaGroups, it.next()) {
+    mbar_wait(bar_full + 8 * g, fph);
+    fph ^= 1u;
+    // ---- conv0.0: 9 K=16 steps (the layer's tap order), each over the kC0MB row blocks
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 9; ++j) {
+      const uint4 d = p.mma0[j];
+      const uint64_t b64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b0_lo + d.z);
+#pragma unroll
+      for (int mb = 0; mb < kC0MB; ++mb)
+        wgmma_ss<32, T>(acc0[mb], ((uint64_t)d.y << 32) | (uint64_t)(x_lo + d.x + 512u * mb), b64, j ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * g);  // the x window may refill
+#pragma unroll
+    for (int mb = 0; mb < kC0MB; ++mb) acc_fence(acc0[mb]);
+
+    // ---- conv0.0 epilogue into the conv0.1 window: row m = 16 wq + 8 e + px of block mb is window row L
+    const int hy0 = 2 * kC0Tile * it.ty - 3, hx0 = 2 * kC0Tile * it.tx - 3;  // x / conv0.0 cell of window (0, 0)
+#pragma unroll
+    for (int mb = 0; mb < kC0MB; ++mb)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int L = kC0XW + 1 + 64 * mb + 16 * wq + 8 * e + px;
+        const int wr = L / kC0XW, wc = L - wr * kC0XW;
+        if (wc == 0 || wr > 2 * kC0Tile + 2) continue;  // (wr, wc in [1, 18])
+        const int hy = hy0 + wr, hx = hx0 + wc;
+        const bool inside = hy >= 0 && hy < H2 && hx >= 0 && hx < W2;
+        const uint32_t cell = (uint32_t)(((wr - 1) >> 1) * (kC0Tile + 1) + ((wc - 1) >> 1));
+        const uint32_t base = c00 + (((wr - 1) & 1) ? p.c00_kb1 : 0u) + 4u * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float a0 = acc0[mb][4 * j + 2 * e] + sh0[j].x, a1 = acc0[mb][4 * j + 2 * e + 1] + sh0[j].y;
+          const uint32_t v = inside ? Pack2<T>::pack(fmaxf(a0, 0.2f * a0), fmaxf(a1, 0.2f * a1)) : 0u;
+          st_shared_u32(base + swz_off(cell, (uint32_t)(((wc - 1) & 1) * 4 + j), 128u), v);
+        }
+      }
+    fence_proxy_async();  // the generic-proxy window writes before the tensor cores read them
+    named_bar_sync(1 + g, 128);
+
+    // ---- conv0.1 on that window: one m64 row block, 9 runs of 2 K=16 steps
+    wgmma_fence();
+#pragma unroll
+    for (int r = 0; r < 9; ++r) {
+      const uint4 d = p.mma1[r];
+      const uint64_t a64 = ((uint64_t)d.y << 32) | (uint64_t)(c00_lo + d.x);
+      const uint64_t b64 = ((uint64_t)p.b_hi << 32) | (uint64_t)(b1_lo + d.z);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) wgmma_ss<64, T>(acc1, a64 + 2u * i, b64 + 2u * i, (r | i) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc1);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      acc1[4 * j] += sh1[j].x;
+      acc1[4 * j + 1] += sh1[j].y;
+      acc1[4 * j + 2] += sh1[j].x;
+      acc1[4 * j + 3] += sh1[j].y;
+    }
+    if (leader) bulk_wait_read<0>();  // the previous tile's store has read the staging tile
+    named_bar_sync(1 + g, 128);      // (also: every warp's conv0.1 MMAs are done before the next tile rewrites the window)
+    stage_rows<64, T>(acc1, out_smem, kC0OutBytes, 2 * wq, lane, 0.2f);
+    fence_proxy_async();
+    named_bar_sync(1 + g, 128);
+    if (leader) {
+      tma_store_4d(&p.tm_out, out_smem, 0, kC0Tile * it.tx, kC0Tile * it.ty, it.b);
+      bulk_commit();
+    }
+  }
+  if (leader) bulk_wait<0>();
+}
 #endif  // VFI_HOST_EMU
 
 // ---------------------------------------------------------------------------------------------
@@ -690,8 +924,6 @@ bool make_tmap(CUtensorMap* tm, CUtensorMapDataType dt, const void* base, int C,
 }
 
 #endif  // VFI_HOST_EMU
-
-uint32_t align_up(uint32_t v, uint32_t a) { return (v + a - 1) / a * a; }
 
 }  // namespace
 
@@ -935,6 +1167,80 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
   };
   err = (op_type == OP_BF16) ? pick(__nv_bfloat16{}) : pick(__half{});
   if (err != cudaSuccess) return err;
+  return cudaGetLastError();
+#endif  // VFI_HOST_EMU
+}
+
+int conv0_fused_plan(const TapConvLayer& L0, const TapConvLayer& L1, int op_type, int* smem_bytes, int* regs,
+                     int* local_bytes) {
+  Conv0Params p{};
+  if (!conv0_fused_layout(L0, L1, &p)) return 0;
+  int r = 0, lb = 0;
+#ifndef VFI_HOST_EMU
+  cudaFuncAttributes fa{};
+  const void* kern = op_type == OP_BF16 ? (const void*)conv0_fused_kernel<__nv_bfloat16> : (const void*)conv0_fused_kernel<__half>;
+  if ((regs || local_bytes) && cudaFuncGetAttributes(&fa, kern) == cudaSuccess) {
+    r = fa.numRegs;
+    lb = (int)fa.localSizeBytes;
+  }
+#else
+  (void)op_type;
+#endif
+  if (smem_bytes) *smem_bytes = (int)p.smem_bytes;
+  if (regs) *regs = r;
+  if (local_bytes) *local_bytes = lb;
+  return kMmaGroups;  // x window stages: one per MMA warpgroup
+}
+
+cudaError_t launch_conv0_fused(const TapConvLayer& L0, const TapConvLayer& L1, int op_type, const void* x, void* c00,
+                               void* out, int B, int H, int W, int num_sms, cudaStream_t st) {
+  Conv0Params p{};
+  if (!conv0_fused_layout(L0, L1, &p)) {
+    set_error("conv0 fused: the layers are not a 64-channel arch-4.6 conv0.0 / conv0.1 pair");
+    return cudaErrorInvalidConfiguration;
+  }
+  if (B < 1 || H < 2 || W < 2 || ((H | W) & 1)) {
+    set_error("conv0 fused: the conv0.0 grid needs even H and W");
+    return cudaErrorInvalidValue;
+  }
+#ifdef VFI_HOST_EMU
+  // the host emulation has only the checker kernel: the two launches, through c00
+  if (!c00) return cudaErrorInvalidValue;
+  const cudaError_t e = launch_tapconv(L0, op_type, x, c00, nullptr, nullptr, B, H, W, num_sms, TAPCONV_CHECKER, st);
+  if (e != cudaSuccess) return e;
+  return launch_tapconv(L1, op_type, c00, out, nullptr, nullptr, B, H / 2, W / 2, num_sms, TAPCONV_CHECKER, st);
+#else
+  (void)c00;
+  const CUtensorMapDataType dt = (op_type == OP_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  p.H4 = H / 2;
+  p.W4 = W / 2;
+  if (!make_tmap(&p.tm_x, dt, x, 64, W, H, B, 64, kC0XW, kC0XW, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_tmap(&p.tm_out, dt, out, 64, p.W4, p.H4, B, 64, kC0Tile, kC0Tile, CU_TENSOR_MAP_SWIZZLE_128B))
+    return cudaErrorInvalidValue;
+  p.w0 = L0.w;
+  p.w1 = L1.w;
+  p.shift0 = L0.shift;
+  p.shift1 = L1.shift;
+  p.B = B;
+  p.tiles_y = (p.H4 + kC0Tile - 1) / kC0Tile;
+  p.tiles_x = (p.W4 + kC0Tile - 1) / kC0Tile;
+  p.ntiles = B * p.tiles_y * p.tiles_x;
+  p.ctas = std::max(1, std::min(num_sms, p.ntiles));
+  auto kern = (op_type == OP_BF16) ? conv0_fused_kernel<__nv_bfloat16> : conv0_fused_kernel<__half>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
+  if (e != cudaSuccess) return e;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)p.ctas);
+  cfg.blockDim = dim3((unsigned)kThreads);
+  cfg.dynamicSmemBytes = p.smem_bytes;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  e = cudaLaunchKernelEx(&cfg, kern, p);
+  if (e != cudaSuccess) return e;
   return cudaGetLastError();
 #endif  // VFI_HOST_EMU
 }

@@ -116,6 +116,14 @@ cudaError_t launch_tapconv(const TapConvLayer& L, int op_type, const void* in, v
                            float* out_mask, int B, int H, int W, int num_sms, int impl, cudaStream_t st);
 // smem/stage plan for a layer (for DESIGN.md tables and tests); returns 0 stages when it cannot fit
 int tapconv_plan(const TapConvLayer& L, TapConvParams* p_out);
+// conv0.0 (L0) and conv0.1 (L1) of a 64-channel arch-4.6 IFBlock as one launch (tapconv.cu): x [B, H, W, 64] -> out
+// [B, H/2, W/2, 64], conv0.0's output kept in shared memory.  The host emulation runs the two checker launches through
+// c00 instead.  conv0_fused_plan returns its x window stages (0: the pair is not of that shape) and its shared-memory
+// bytes, registers per thread and local (spill) bytes per thread.
+int conv0_fused_plan(const TapConvLayer& L0, const TapConvLayer& L1, int op_type, int* smem_bytes, int* regs,
+                     int* local_bytes);
+cudaError_t launch_conv0_fused(const TapConvLayer& L0, const TapConvLayer& L1, int op_type, const void* x, void* c00,
+                               void* out, int B, int H, int W, int num_sms, cudaStream_t st);
 
 // imgs: fp32 float4 planes (final blend); imgs_h: the same pixels as half4 (8 bytes) for the block-input warps, whose
 // results are rounded to 16 bits anyway - half the gather bytes through L1

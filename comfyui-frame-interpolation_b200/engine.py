@@ -164,6 +164,22 @@ class Rife46Engine:
         return dict(stages=st.value, n_cta=nc.value, nsplit=ns.value, smem_bytes=sm.value, macs_per_cell=mc.value,
                     cmajor=bool(cm.value), wstream=bool(ws.value))
 
+    def debug_conv0_fused(self, block, x, out):
+        """conv0.0 -> conv0.1 of `block` as the one fused launch: x [B,H,W,64] 16-bit -> out [B,H/2,W/2,64] 16-bit."""
+        b, h, w = x.shape[0], x.shape[1], x.shape[2]
+        st = torch.cuda.current_stream(x.device).cuda_stream
+        check(self._L.vfi_rife46_debug_conv0_fused(self._ctx, block, x.data_ptr(), out.data_ptr(), b, h, w, st))
+        return out
+
+    def set_unfused_conv0(self, unfused: bool):
+        """Test hook: run every block's conv0.0 and conv0.1 as two launches (True) or fused where possible (False)."""
+        check(self._L.vfi_rife46_debug_unfused_conv0(self._ctx, 1 if unfused else 0))
+
+    def conv0_plan(self, block):
+        v = np.zeros(5, np.int32)
+        check(self._L.vfi_rife46_conv0_plan(self._ctx, block, v.ctypes.data, 5))
+        return dict(fused=bool(v[0]), stages=int(v[1]), smem_bytes=int(v[2]), regs=int(v[3]), local_bytes=int(v[4]))
+
     def debug_state(self, batch):
         """(flow [B,Hp,Wp,4], mask [B,Hp,Wp]) of the last internal pass as torch CUDA tensors."""
         hp, wp = C.c_int(), C.c_int()

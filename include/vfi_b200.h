@@ -347,6 +347,16 @@ int vfi_rife46_debug_state(vfi_ctx* ctx, float* flow4_out, float* mask_out, int 
  * wstream = 1 when its weights stream through shared memory instead of staying resident (any pointer may be NULL). */
 int vfi_rife46_layer_plan(vfi_ctx* ctx, int block, int layer, int* stages, int* n_cta, int* nsplit, int* smem_bytes,
                           int64_t* macs_per_cell, int* cmajor, int* wstream);
+/* conv0.0 and conv0.1 of arch 4.6's 64-channel block (block 3) run as one launch whenever that block runs at full
+ * resolution (scale 1): conv0.0's output stays in shared memory (DESIGN.md section 4.1).  vfi_rife46_debug_conv0_fused
+ * runs that launch alone over `in` (the block input, 16-bit [B, H, W, 64] space-to-depth cells) into `out` (16-bit
+ * [B, H/2, W/2, 64]); VFI_E_INVALID for a block whose layers it cannot run.  vfi_rife46_debug_unfused_conv0(ctx, 1) makes
+ * the forward schedule run that block's conv0.0 and conv0.1 as two launches instead (0: back to one), the tests'
+ * reference.  vfi_rife46_conv0_plan: info[0..4] = {1 when the block's pair can run fused (at scale 1), its x window
+ * stages, shared-memory bytes, registers per thread, local (spill) bytes per thread}, all 0 otherwise (at most cap). */
+int vfi_rife46_debug_conv0_fused(vfi_ctx* ctx, int block, const void* in, void* out, int B, int H, int W, void* stream);
+int vfi_rife46_debug_unfused_conv0(vfi_ctx* ctx, int unfused);
+int vfi_rife46_conv0_plan(vfi_ctx* ctx, int block, int32_t* info, int cap);
 int vfi_sync(vfi_ctx* ctx);
 /* Run ONE streamconv layer (csrc/streamconv.cu, the conv kernel of FILM, Sepconv, FLAVR, IFRNet and CAIN) from a plain
  * description, without a model: spec = {ksize, c0, c1, n_total, act, ext, n_f32, pad_before, pad_before_x, kt, pad_t,
