@@ -1,4 +1,4 @@
-"""CPU restatement (fp32) of GMFlow as GMFSS Fortuna uses it - SURVEY.md section 8 row a11.  TEST INFRASTRUCTURE ONLY; GMFSS is
+"""CPU restatement of GMFlow as GMFSS Fortuna uses it - SURVEY.md section 8 row a11.  TEST INFRASTRUCTURE ONLY; GMFSS is
 not built in this repo yet, this file and oracle/gmfss.py pin its target.
 
 Follows ``vfi_models/gmfss_fortuna/GMFSS_Fortuna_union_arch.py`` of Fannovel16/ComfyUI-Frame-Interpolation @ 26545cc, the
@@ -17,6 +17,10 @@ inference configuration ``Model.reuse`` :1726-1782 runs (``GMFlow()`` defaults :
 * ``gmflow``           GMFlow.forward :1262-1369.
 
 Pinned by tests/test_oracle_gmfss.py against the flows of the unmodified reference (tests/golden/gmfss_*.npz).
+
+Every tensor it creates takes the dtype and device of its inputs: fp32 CPU tensors give the fp32 restatement the goldens pin,
+float64 tensors on any device the float64 reference tests/test_gpu_zgmfss_shadow.py compares
+the product with.
 """
 from __future__ import annotations
 
@@ -73,12 +77,12 @@ def _unwindows_last(x, k: int):
     return x.view(b, k, k, h, w, c).permute(0, 1, 3, 2, 4, 5).contiguous().view(b, k * h, k * w, c)
 
 
-def position_sine(b: int, h: int, w: int, feats: int = 64, temperature: float = 10000.0):
-    ones = torch.ones(b, h, w)
-    ye, xe = ones.cumsum(1, dtype=torch.float32), ones.cumsum(2, dtype=torch.float32)
+def position_sine(b: int, h: int, w: int, feats: int = 64, temperature: float = 10000.0, dtype=torch.float32, device=None):
+    ones = torch.ones(b, h, w, dtype=dtype, device=device)
+    ye, xe = ones.cumsum(1, dtype=dtype), ones.cumsum(2, dtype=dtype)
     ye = ye / (ye[:, -1:, :] + 1e-6) * (2 * math.pi)
     xe = xe / (xe[:, :, -1:] + 1e-6) * (2 * math.pi)
-    dim_t = torch.arange(feats, dtype=torch.float32)
+    dim_t = torch.arange(feats, dtype=dtype, device=device)
     dim_t = temperature ** (2 * (dim_t // 2) / feats)
     px, py = xe[:, :, :, None] / dim_t, ye[:, :, :, None] / dim_t
     px = torch.stack((px[:, :, :, 0::2].sin(), px[:, :, :, 1::2].cos()), dim=4).flatten(3)
@@ -88,14 +92,14 @@ def position_sine(b: int, h: int, w: int, feats: int = 64, temperature: float = 
 
 def add_position(f0, f1, splits: int):
     a, b = _windows(f0, splits), _windows(f1, splits)
-    pos = position_sine(a.shape[0], a.shape[2], a.shape[3], f0.shape[1] // 2)
+    pos = position_sine(a.shape[0], a.shape[2], a.shape[3], f0.shape[1] // 2, dtype=f0.dtype, device=f0.device)
     return _unwindows(a + pos, splits), _unwindows(b + pos, splits)
 
 
-def shift_mask(h: int, w: int, splits: int):
+def shift_mask(h: int, w: int, splits: int, dtype=torch.float32, device=None):
     wh, ww = h // splits, w // splits
     sh, sw = wh // 2, ww // 2
-    img = torch.zeros(1, h, w, 1)
+    img = torch.zeros(1, h, w, 1, dtype=dtype, device=device)
     cnt = 0
     for hs in (slice(0, -wh), slice(-wh, -sh), slice(-sh, None)):
         for ws in (slice(0, -ww), slice(-ww, -sw), slice(-sw, None)):
@@ -144,7 +148,7 @@ def transformer(sd, f0, f1, splits: int, num_layers: int = 6):
     b, c, h, w = f0.shape
     a = f0.flatten(-2).permute(0, 2, 1)
     bb = f1.flatten(-2).permute(0, 2, 1)
-    mask = shift_mask(h, w, splits) if splits > 1 else None
+    mask = shift_mask(h, w, splits, f0.dtype, f0.device) if splits > 1 else None
     c0, c1 = torch.cat((a, bb), 0), torch.cat((bb, a), 0)
     for i in range(num_layers):
         p = f"transformer.layers.{i}"
@@ -156,30 +160,30 @@ def transformer(sd, f0, f1, splits: int, num_layers: int = 6):
     return (a.view(b, h, w, c).permute(0, 3, 1, 2).contiguous(), bb.view(b, h, w, c).permute(0, 3, 1, 2).contiguous())
 
 
-def _grid(b: int, h: int, w: int):
-    y, x = torch.meshgrid(torch.arange(h), torch.arange(w), indexing="ij")
-    return torch.stack([x, y], 0).float()[None].repeat(b, 1, 1, 1)
+def _grid(b: int, h: int, w: int, dtype=torch.float32, device=None):
+    y, x = torch.meshgrid(torch.arange(h, device=device), torch.arange(w, device=device), indexing="ij")
+    return torch.stack([x, y], 0).to(dtype)[None].repeat(b, 1, 1, 1)
 
 
 def global_match(f0, f1):
     b, c, h, w = f0.shape
     corr = torch.matmul(f0.view(b, c, -1).permute(0, 2, 1), f1.view(b, c, -1)).view(b, h, w, h, w) / c ** 0.5
-    init = _grid(b, h, w)
+    init = _grid(b, h, w, f0.dtype, f0.device)
     prob = F.softmax(corr.view(b, h * w, h * w), dim=-1)
     return torch.matmul(prob, init.view(b, 2, -1).permute(0, 2, 1)).view(b, h, w, 2).permute(0, 3, 1, 2) - init
 
 
 def local_match(f0, f1, radius: int):
     b, c, h, w = f0.shape
-    init = _grid(b, h, w)
+    init = _grid(b, h, w, f0.dtype, f0.device)
     coords = init.view(b, 2, -1).permute(0, 2, 1)
     k = 2 * radius + 1
-    lin = torch.linspace(-radius, radius, k)
+    lin = torch.linspace(-radius, radius, k, dtype=f0.dtype, device=f0.device)
     gx, gy = torch.meshgrid([lin, lin], indexing="ij")
-    window = torch.stack((gx, gy), -1).transpose(0, 1).float().reshape(-1, 2).repeat(b, 1, 1, 1)
+    window = torch.stack((gx, gy), -1).transpose(0, 1).reshape(-1, 2).repeat(b, 1, 1, 1)
     sample = coords.unsqueeze(-2) + window                                             # [B, H*W, k*k, 2]
     valid = (sample[..., 0] >= 0) & (sample[..., 0] < w) & (sample[..., 1] >= 0) & (sample[..., 1] < h)
-    half = torch.tensor([(w - 1) / 2.0, (h - 1) / 2.0])
+    half = torch.tensor([(w - 1) / 2.0, (h - 1) / 2.0], dtype=f0.dtype, device=f0.device)
     feat = F.grid_sample(f1, (sample - half) / half, padding_mode="zeros", align_corners=True).permute(0, 2, 1, 3)
     corr = torch.matmul(f0.permute(0, 2, 3, 1).reshape(b, h * w, 1, c), feat).view(b, h * w, -1) / c ** 0.5
     corr[~valid] = -1e9
@@ -215,15 +219,15 @@ def upsample_convex(sd, flow, feature, factor: int = 4):
 
 def _warp(feature, flow):
     b, c, h, w = feature.shape
-    co = _grid(b, h, w) + flow
+    co = _grid(b, h, w, flow.dtype, flow.device) + flow
     g = torch.stack([2 * co[:, 0] / (w - 1) - 1, 2 * co[:, 1] / (h - 1) - 1], -1)
     return F.grid_sample(feature, g, mode="bilinear", padding_mode="zeros", align_corners=True)
 
 
 def gmflow(sd, img0, img1):
     """Flow img0 -> img1 at the images' resolution (images in [0, 1], sides multiples of 32)."""
-    mean = torch.tensor([0.485, 0.456, 0.406]).view(1, 3, 1, 1)
-    std = torch.tensor([0.229, 0.224, 0.225]).view(1, 3, 1, 1)
+    mean = torch.tensor([0.485, 0.456, 0.406], dtype=img0.dtype, device=img0.device).view(1, 3, 1, 1)
+    std = torch.tensor([0.229, 0.224, 0.225], dtype=img0.dtype, device=img0.device).view(1, 3, 1, 1)
     feats = encoder(sd, torch.cat(((img0 - mean) / std, (img1 - mean) / std), 0))[::-1]     # low to high resolution
     flow = None
     for scale, (splits, corr_radius, prop_radius) in enumerate(((2, -1, -1), (8, 4, 1))):

@@ -1,4 +1,4 @@
-"""CPU restatement (fp32) of GMFSS Fortuna (union) around its flow network (oracle/gmflow.py) - SURVEY.md section 8 row a11.
+"""CPU restatement of GMFSS Fortuna (union) around its flow network (oracle/gmflow.py) - SURVEY.md section 8 row a11.
 TEST INFRASTRUCTURE ONLY; GMFSS is not built in this repo yet, this file pins most of its target.
 
 Follows ``vfi_models/gmfss_fortuna/GMFSS_Fortuna_union_arch.py`` of Fannovel16/ComfyUI-Frame-Interpolation @ 26545cc:
@@ -11,6 +11,7 @@ tests/test_ops_ref_pinned.py), ``GMFlow`` (:35-1372, the transformer flow networ
 reference's flows, so everything downstream of GMFlow is pinned on its own (tests/test_oracle_gmfss.py: metrics and the frame
 from the golden flows), GMFlow on its own (the flows), and ``interpolate`` - the whole model as
 ``CommonModelInference.forward`` (gmfss_fortuna/__init__.py:41-77) runs it at scale 1 - end to end (the frame from the images).
+Like oracle/gmflow.py it computes in the dtype and on the device of its inputs (fp32 or float64).
 """
 from __future__ import annotations
 
@@ -27,8 +28,8 @@ from . import rife46 as R
 def backwarp(ten_in: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     """:1375-1417: grid_sample(bilinear, zeros, align_corners=True) at pixel + flow."""
     h, w = flow.shape[2], flow.shape[3]
-    hor = torch.linspace(-1.0, 1.0, w).view(1, 1, 1, -1).repeat(1, 1, h, 1)
-    ver = torch.linspace(-1.0, 1.0, h).view(1, 1, -1, 1).repeat(1, 1, 1, w)
+    hor = torch.linspace(-1.0, 1.0, w, dtype=flow.dtype, device=flow.device).view(1, 1, 1, -1).repeat(1, 1, h, 1)
+    ver = torch.linspace(-1.0, 1.0, h, dtype=flow.dtype, device=flow.device).view(1, 1, -1, 1).repeat(1, 1, 1, w)
     grid = torch.cat([hor, ver], 1)
     fl = torch.cat([flow[:, 0:1] / ((ten_in.shape[3] - 1.0) / 2.0), flow[:, 1:2] / ((ten_in.shape[2] - 1.0) / 2.0)], 1)
     return F.grid_sample(ten_in, (grid + fl).permute(0, 2, 3, 1), mode="bilinear", padding_mode="zeros", align_corners=True)
@@ -37,8 +38,8 @@ def backwarp(ten_in: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
 def _flow_warp(feature: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     """flow_warp :985-991 + bilinear_sample :955-983 (padding 'zeros', align_corners=True) + coords_grid :916-932."""
     b, c, h, w = feature.shape
-    y, x = torch.meshgrid(torch.arange(h), torch.arange(w), indexing="ij")
-    coords = torch.stack([x, y], 0).float()[None].repeat(b, 1, 1, 1) + flow
+    y, x = torch.meshgrid(torch.arange(h, device=flow.device), torch.arange(w, device=flow.device), indexing="ij")
+    coords = torch.stack([x, y], 0).to(flow.dtype)[None].repeat(b, 1, 1, 1) + flow
     xg = 2 * coords[:, 0] / (w - 1) - 1
     yg = 2 * coords[:, 1] / (h - 1) - 1
     return F.grid_sample(feature, torch.stack([xg, yg], -1), mode="bilinear", padding_mode="zeros", align_corners=True)
@@ -50,7 +51,7 @@ def fb_consistency(fwd: torch.Tensor, bwd: torch.Tensor, alpha: float = 0.01, be
     diff_f = torch.norm(fwd + _flow_warp(bwd, fwd), dim=1)
     diff_b = torch.norm(bwd + _flow_warp(fwd, bwd), dim=1)
     thr = alpha * mag + beta
-    return (diff_f > thr).float(), (diff_b > thr).float()
+    return (diff_f > thr).to(fwd.dtype), (diff_b > thr).to(fwd.dtype)
 
 
 def _pconv(sd, prefix: str, x: torch.Tensor, stride: int = 1) -> torch.Tensor:
@@ -131,16 +132,20 @@ def reuse_from_flows(sds: Dict[str, dict], img0, img1, flow01, flow10):
     return m0, m1, f1, f2
 
 
-def inference(sds: Dict[str, dict], img0, img1, flow01, flow10, metric0, metric1, f1, f2, timestep: float) -> torch.Tensor:
-    """Model.inference :1784-1857."""
+def inference(sds: Dict[str, dict], img0, img1, flow01, flow10, metric0, metric1, f1, f2, timestep: float, rife=None) -> torch.Tensor:
+    """Model.inference :1784-1857.  `rife` (h0, h1, t) -> merged frame stands in for the IFNet 4.6 sub-model when given
+    (e.g. another implementation's output, so that the rest of the model can be compared on its own)."""
     splat = lambda a, fl, z: ops_ref.softsplat(a, fl, z, "soft")   # noqa: E731
     dn = lambda a, s: F.interpolate(a, scale_factor=s, mode="bilinear", align_corners=False)   # noqa: E731
     F1t, F2t = timestep * flow01, (1 - timestep) * flow10
     Z1t, Z2t = timestep * metric0, (1 - timestep) * metric1
     h0, h1 = dn(img0, 0.5), dn(img1, 0.5)
     I1t, I2t = splat(h0, F1t, Z1t), splat(h1, F2t, Z2t)
-    ts = torch.full((img0.shape[0], 1, 1, 1), float(timestep))
-    rife = R.ifnet46_forward(sds["ifnet"], h0, h1, ts, (8, 4, 2, 1))
+    if rife is None:
+        ts = torch.full((img0.shape[0], 1, 1, 1), float(timestep))
+        rife = R.ifnet46_forward(sds["ifnet"], h0, h1, ts, (8, 4, 2, 1))
+    else:
+        rife = rife(h0, h1, timestep)
     a1, b1 = splat(f1[0], F1t, Z1t), splat(f2[0], F2t, Z2t)
     a2, b2 = splat(f1[1], dn(F1t, 0.5) * 0.5, dn(Z1t, 0.5)), splat(f2[1], dn(F2t, 0.5) * 0.5, dn(Z2t, 0.5))
     a3, b3 = splat(f1[2], dn(F1t, 0.25) * 0.25, dn(Z1t, 0.25)), splat(f2[2], dn(F2t, 0.25) * 0.25, dn(Z2t, 0.25))
@@ -157,11 +162,11 @@ def reuse(sds: Dict[str, dict], img0, img1):
     return (flow01, flow10) + tuple(reuse_from_flows(sds, img0, img1, flow01, flow10))
 
 
-def interpolate(sds: Dict[str, dict], frame0, frame1, timestep: float) -> torch.Tensor:
+def interpolate(sds: Dict[str, dict], frame0, frame1, timestep: float, rife=None) -> torch.Tensor:
     """CommonModelInference.forward, gmfss_fortuna/__init__.py:41-77, scale 1: pad to multiples of 64 at the bottom / right,
-    reuse + inference, crop."""
+    reuse + inference (`rife` as there), crop."""
     h, w = frame0.shape[2], frame0.shape[3]
     ph, pw = ((h - 1) // 64 + 1) * 64, ((w - 1) // 64 + 1) * 64
     i0, i1 = F.pad(frame0, (0, pw - w, 0, ph - h)), F.pad(frame1, (0, pw - w, 0, ph - h))
     flow01, flow10, m0, m1, f1, f2 = reuse(sds, i0, i1)
-    return inference(sds, i0, i1, flow01, flow10, m0, m1, f1, f2, timestep)[:, :, :h, :w]
+    return inference(sds, i0, i1, flow01, flow10, m0, m1, f1, f2, timestep, rife)[:, :, :h, :w]

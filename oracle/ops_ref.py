@@ -19,10 +19,12 @@ def softsplat_sum(ten_in: torch.Tensor, ten_flow: torch.Tensor) -> torch.Tensor:
     Each source pixel (n,c,y,x) adds in*w to its four bilinear neighbours of (x+fx, y+fy); targets outside the image
     are dropped; a non-finite flow drops the pixel.  The reference uses atomicAdd (order nondeterministic); here the
     sum is accumulated with index_add_ in float64 and rounded once, so agreement with any summation order is ~1 ulp
-    of the partial sums."""
+    of the partial sums.  The corner weights are computed in the flow's dtype and the result is returned in the input's
+    (fp32 like the reference, or float64 throughout), on the inputs' device."""
     n, c, h, w = ten_in.shape
-    out = torch.zeros(n, c, h * w, dtype=torch.float64)
-    ys, xs = torch.meshgrid(torch.arange(h, dtype=torch.float32), torch.arange(w, dtype=torch.float32), indexing="ij")
+    dt, dev = ten_flow.dtype, ten_flow.device
+    out = torch.zeros(n, c, h * w, dtype=torch.float64, device=dev)
+    ys, xs = torch.meshgrid(torch.arange(h, dtype=dt, device=dev), torch.arange(w, dtype=dt, device=dev), indexing="ij")
     for b in range(n):
         fx = xs + ten_flow[b, 0]
         fy = ys + ten_flow[b, 1]
@@ -40,9 +42,9 @@ def softsplat_sum(ten_in: torch.Tensor, ten_flow: torch.Tensor) -> torch.Tensor:
             wgt = (wx * wy)
             inside = ok & (tx >= 0) & (tx < w) & (ty >= 0) & (ty < h)
             idx = (ty.clamp(0, h - 1) * w + tx.clamp(0, w - 1)).long().reshape(-1)
-            contrib = (src.float() * wgt.reshape(1, -1)).double() * inside.reshape(1, -1)
+            contrib = (src.to(dt) * wgt.reshape(1, -1)).double() * inside.reshape(1, -1)
             out[b].index_add_(1, idx, contrib)
-    return out.reshape(n, c, h, w).float()
+    return out.reshape(n, c, h, w).to(ten_in.dtype)
 
 
 def softsplat(ten_in, ten_flow, ten_metric, mode: str):
